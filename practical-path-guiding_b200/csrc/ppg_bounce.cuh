@@ -9,11 +9,11 @@ namespace ppg {
 // RECORD: 0 = no vertex records (final iteration), 1 = basic record (nearest spatial filter, no loss),
 //         2 = full record (stochastic/box spatial filter or a sampling-fraction loss).
 template <bool FIRST, int RECORD, bool NEE, bool SMEM, bool FULL>
-__global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM, SMEM ? PPG_MIN_BLOCKS : PPG_MIN_BLOCKS_HBM) bounce_kernel(const RenderParams P) {
+__global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM, SMEM ? PPG_MIN_BLOCKS : PPG_MIN_BLOCKS_HBM) bounce_kernel(const __grid_constant__ RenderParams P) {
     const SceneAccess<SMEM> sc(P.scene);
     sc.stage();
     const uint32_t nIn = FIRST ? P.nPaths : *P.liveIn;
-    unsigned long long raysLocal = 0, recLocal = 0, levelsLocal = 0;
+    uint32_t raysLocal = 0, recLocal = 0, levelsLocal = 0;          // per thread: 32 bits hold a launch's worth; widened for the warp sum
     // material bins left by trace_kernel: position j of the launch is the (j - start)-th entry of the bin that contains it
     __shared__ uint32_t binStart[PPG_BINS + 1];
     const bool binned = !SMEM && P.order != nullptr;
@@ -43,11 +43,12 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
         }
         float3 o, d, thr, Li; float eta = 1.f, rrRecip = 1.f, mint, maxt;
         float prevWoPdf = 0.f; float3 prevRefN = f3(0, 0, 0); uint32_t prevSlot = 0;      // NEE only
-        uint32_t pathId = 0, nVertices = 0, flags = 0; uint64_t sampleIndex = 0;
-        Pcg32 rng; rng.state = 0; rng.inc = 1;
+        uint32_t pathId = 0, nVertices = 0, flags = 0;
+        Pcg32 rng; rng.state = 0; rng.inc = 1;        // the path's stream is keyed by its sample index: rng.inc == 2 * sampleIndex + 1
         if (alive) {
             if (FIRST) {
                 pathId = i;
+                uint64_t sampleIndex;
                 camera_ray(P, i, rng, sampleIndex, o, d, mint, maxt);
                 thr = f3(1, 1, 1); Li = f3(0, 0, 0);
             } else {
@@ -55,7 +56,7 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                 o = f3(a.x, a.y, a.z); d = f3(a.w, b.x, b.y); thr = f3(b.z, b.w, c.x); eta = c.y; Li = f3(c.z, c.w, e.x);
                 pathId = __float_as_uint(e.y);
                 rng.state = ((uint64_t) __float_as_uint(e.w) << 32) | __float_as_uint(e.z);
-                sampleIndex = ((uint64_t) __float_as_uint(f.y) << 32) | __float_as_uint(f.x);
+                const uint64_t sampleIndex = ((uint64_t) __float_as_uint(f.y) << 32) | __float_as_uint(f.x);
                 rng.inc = (sampleIndex << 1) | 1u;
                 const uint32_t nf = __float_as_uint(f.z); nVertices = nf & 0xffu; flags = nf >> 8;
                 rrRecip = f.w;
@@ -238,7 +239,7 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                                     __stcs(&P.neeSlab.v2[i], make_float4(L.x, L.y, L.z, __uint_as_float(pathId | 0x40000000u)));   // bit 30: absolute radiance
                                     __stcs(&P.neeSlab.v3[i], make_float4(bsdfVal.x, bsdfVal.y, bsdfVal.z, nBsdfPdf));
                                     __stcs(&P.neeSlab.v4[i], make_float4(its.p.x, its.p.y, its.p.z, nDTreePdf));
-                                    __stcs(&P.neeSlab.v5[i], make_float4(__uint_as_float((uint32_t) sampleIndex), __uint_as_float((uint32_t) (sampleIndex >> 32)),
+                                    __stcs(&P.neeSlab.v5[i], make_float4(__uint_as_float((uint32_t) (rng.inc >> 1)), __uint_as_float((uint32_t) (rng.inc >> 33)),
                                                                   __uint_as_float((uint32_t) levels | ((32u + (uint32_t) P.depth) << 8)), 0.f));
                                     wroteNee = true;
                                 }
@@ -265,7 +266,7 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                             const float3 bv = bsdfWeight * woPdf;
                             __stcs(&P.slab.v3[i], make_float4(bv.x, bv.y, bv.z, bsdfPdf));
                             __stcs(&P.slab.v4[i], make_float4(o.x, o.y, o.z, dTreePdf));
-                            __stcs(&P.slab.v5[i], make_float4(__uint_as_float((uint32_t) sampleIndex), __uint_as_float((uint32_t) (sampleIndex >> 32)),
+                            __stcs(&P.slab.v5[i], make_float4(__uint_as_float((uint32_t) (rng.inc >> 1)), __uint_as_float((uint32_t) (rng.inc >> 33)),
                                                        __uint_as_float((uint32_t) levels | (nVertices << 8)), 0.f));
                         }
                         wroteVertex = true; ++nVertices; ++recLocal; levelsLocal += levels;
@@ -298,7 +299,7 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
             __stcs(&P.out.s1[slot], make_float4(d.y, d.z, thr.x, thr.y));
             __stcs(&P.out.s2[slot], make_float4(thr.z, eta, Li.x, Li.y));
             __stcs(&P.out.s3[slot], make_float4(Li.z, __uint_as_float(pathId), __uint_as_float((uint32_t) rng.state), __uint_as_float((uint32_t) (rng.state >> 32))));
-            __stcs(&P.out.s4[slot], make_float4(__uint_as_float((uint32_t) sampleIndex), __uint_as_float((uint32_t) (sampleIndex >> 32)),
+            __stcs(&P.out.s4[slot], make_float4(__uint_as_float((uint32_t) (rng.inc >> 1)), __uint_as_float((uint32_t) (rng.inc >> 33)),
                                          __uint_as_float(nVertices | (flags << 8)), rrRecip));
             if (NEE) {
                 __stcs(&P.out.s5[slot], make_float4(prevWoPdf, prevRefN.x, prevRefN.y, prevRefN.z));
@@ -307,14 +308,15 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
         }
     }
     // per-warp reduction of the statistics counters
+    unsigned long long rays = raysLocal, rec = recLocal, lev = levelsLocal;
     for (int off = 16; off; off >>= 1) {
-        raysLocal += __shfl_xor_sync(0xffffffffu, raysLocal, off);
-        recLocal += __shfl_xor_sync(0xffffffffu, recLocal, off);
-        levelsLocal += __shfl_xor_sync(0xffffffffu, levelsLocal, off);
+        rays += __shfl_xor_sync(0xffffffffu, rays, off);
+        rec += __shfl_xor_sync(0xffffffffu, rec, off);
+        lev += __shfl_xor_sync(0xffffffffu, lev, off);
     }
     if ((threadIdx.x & 31) == 0) {
-        if (raysLocal) atomicAdd(&P.counters[0], raysLocal);
-        if (recLocal) { atomicAdd(&P.counters[1], recLocal); atomicAdd(&P.counters[2], levelsLocal); }
+        if (rays) atomicAdd(&P.counters[0], rays);
+        if (rec) { atomicAdd(&P.counters[1], rec); atomicAdd(&P.counters[2], lev); }
     }
 }
 

@@ -34,6 +34,14 @@ __device__ __forceinline__ bool is_valid(float3 a) {   // Spectrum::isValid: fin
 }
 __device__ __forceinline__ float max3(float3 a) { return fmaxf(fmaxf(a.x, a.y), a.z); }
 __device__ __forceinline__ float comp(float3 a, int i) { return i == 0 ? a.x : (i == 1 ? a.y : a.z); }
+// sincosf of an angle the caller bounds (|x| <= 2 pi, or NaN): the same result, without sincosf's large-argument reduction
+// (|x| >= 105615), whose scratch array would give every thread of the kernel a local-memory frame
+__device__ __forceinline__ void sincosf_bounded(float x, float *s, float *c) {
+#ifdef __CUDA_ARCH__
+    __builtin_assume(!(fabsf(x) >= 105615.0f));
+#endif
+    sincosf(x, s, c);
+}
 
 // ------------------------------------------------------------------ PCG32 path sampler
 // One stream per path, keyed by (seed, global sample index); numbers are consumed in the
@@ -126,6 +134,7 @@ struct Hit { float t, u, v; uint32_t tri; uint32_t prim; };
 // address was once compiled to LDG and faulted).  SMEM == false reads HBM through the read-only path.
 extern __shared__ float4 ppg_scene_smem[];
 template <bool SMEM> struct SceneAccess {
+    static constexpr bool kStaged = SMEM;
     const SceneView &g;
     uint32_t oGeom, oMeta, oBvh, oBsdf, oRadiance, oGroups;      // float4 offsets of the staged sections (accel at 0)
     __device__ __forceinline__ SceneAccess(const SceneView &v) : g(v) {
@@ -228,21 +237,24 @@ __device__ __forceinline__ bool bvh_slab(float3 o, float3 inv, float mint, float
     return t0 <= t1;
 }
 // Not inlined: the walk's two stacks and its registers stay out of the callers' frames (the tiny-scene path of the bounce
-// kernel never calls it and keeps its register allocation).
-template <class Acc>
-__device__ __noinline__ bool bvh_walk(const Acc &A_, float3 o, float3 d, float mint, float maxt, Hit &hit) {
+// kernel never calls it and keeps its register allocation).  Arguments and result are values: an object whose address is passed to
+// a call that is not inlined has to live in the caller's local memory.  Only the HBM variants walk (staged scenes have coplanar groups).
+static __device__ __noinline__ Hit bvh_walk(const float4 *__restrict__ accel, const float4 *__restrict__ bvh, float3 o, float3 d, float mint, float maxt) {
+    Hit hit; hit.t = __int_as_float(0x7f800000); hit.u = hit.v = 0.f; hit.prim = 0xFFFFFFFFu; hit.tri = 0;
     // BVH walk, near child first.  A node is 2 float4 {min.xyz, bits(left)}, {max.xyz, bits(count)}; siblings are adjacent, so one
     // 64-byte fetch brings both children's boxes.  The far child is pushed with its entry distance and skipped on pop when
     // a closer hit has been found since.  The slab test is widened by 1 ulp-ish factors so that flat boxes and NaNs (0 * inf)
     // never cull; results do not depend on the visiting order (ties on t go to the lower original triangle index).
     const float3 inv = f3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
     auto slab = [&](const float4 n0, const float4 n1, float &tEntry) -> bool { return bvh_slab(o, inv, mint, fminf(maxt, hit.t), n0, n1, tEntry); };
+    auto node = [&](uint32_t i) { return __ldg(&bvh[i]); };
+    auto tri = [&](uint32_t i) { return __ldg(&accel[i]); };
     uint32_t stackN[PPG_BVH_STACK]; float stackT[PPG_BVH_STACK]; int sp = 0;
     uint32_t left, count;      // the current node: children left, left+1 (count == 0) or leaf slots [left, left+count)
     {
-        const float4 r0 = A_.bvh(0), r1 = A_.bvh(1);
+        const float4 r0 = node(0), r1 = node(1);
         float te;
-        if (!slab(r0, r1, te)) return false;
+        if (!slab(r0, r1, te)) return hit;
         left = __float_as_uint(r0.w); count = __float_as_uint(r1.w);
     }
     auto pop = [&]() -> bool {
@@ -258,7 +270,7 @@ __device__ __noinline__ bool bvh_walk(const Acc &A_, float3 o, float3 d, float m
     bool done = false;
     for (;;) {
         while (count == 0u && !done) {
-            const float4 a0 = A_.bvh(2 * left), a1 = A_.bvh(2 * left + 1), b0 = A_.bvh(2 * left + 2), b1 = A_.bvh(2 * left + 3);
+            const float4 a0 = node(2 * left), a1 = node(2 * left + 1), b0 = node(2 * left + 2), b1 = node(2 * left + 3);
             float ta, tb;
             const bool ha = slab(a0, a1, ta), hb = slab(b0, b1, tb);
             if (ha && hb) {
@@ -272,7 +284,7 @@ __device__ __noinline__ bool bvh_walk(const Acc &A_, float3 o, float3 d, float m
         }
         if (done) break;
         for (uint32_t i = left; i < left + count; ++i) {
-            const float4 A = A_.accel(3 * i), B = A_.accel(3 * i + 1), C = A_.accel(3 * i + 2);
+            const float4 A = tri(3 * i), B = tri(3 * i + 1), C = tri(3 * i + 2);
             float u, v, t;
             if (tri_intersect(A, B, C, o, d, mint, maxt, u, v, t)) {
                 const uint32_t prim = __float_as_uint(C.z);
@@ -281,7 +293,7 @@ __device__ __noinline__ bool bvh_walk(const Acc &A_, float3 o, float3 d, float m
         }
         if (!pop()) break;
     }
-    return hit.prim != 0xFFFFFFFFu;
+    return hit;
 }
 template <class Acc> __device__ __forceinline__ bool tri_scene_intersect(const Acc &A_, float3 o, float3 d, float mint, float maxt, Hit &hit);
 
@@ -304,7 +316,7 @@ __device__ __forceinline__ bool tri_scene_intersect(const Acc &A_, float3 o, flo
     const SceneView &sc = A_.g;
     hit.t = __int_as_float(0x7f800000); hit.prim = 0xFFFFFFFFu; hit.tri = 0;
     if (sc.nTris == 0u) return false;
-    if (sc.nGroups != 0u) {      // host sets nGroups only for tiny scenes (<= PPG_BRUTE_FORCE_TRIS triangles in <= 32 coplanar groups)
+    if (Acc::kStaged || sc.nGroups != 0u) {      // host sets nGroups only for tiny scenes (<= PPG_BRUTE_FORCE_TRIS triangles in <= 32 coplanar groups), and stages only those
         // Tiny scenes (CBOX: 36 triangles in 18 coplanar groups, staged in shared memory).  A BVH walk makes every lane
         // of a warp reach its leaves at different times (measured: 2.5 of 32 lanes active in the triangle test), so
         // instead all lanes visit every coplanar group in lock step (shared-memory broadcasts; groups are ordered by
@@ -357,7 +369,8 @@ __device__ __forceinline__ bool tri_scene_intersect(const Acc &A_, float3 o, flo
         }
         return hit.prim != 0xFFFFFFFFu;
     }
-    return bvh_walk(A_, o, d, mint, maxt, hit);
+    hit = bvh_walk(sc.accel, sc.bvh, o, d, mint, maxt);
+    return hit.prim != 0xFFFFFFFFu;
 }
 
 // Intersection record (render/shape.h:36), the fields the path uses
@@ -419,7 +432,7 @@ __device__ __forceinline__ float3 square_to_cosine_hemisphere(float sx, float sy
     if (r1 == 0.f && r2 == 0.f) { r = phi = 0.f; }
     else if (r1 * r1 > r2 * r2) { r = r1; phi = (PPG_PI / 4.0f) * (r2 / r1); }
     else { r = r2; phi = (PPG_PI / 2.0f) - (r1 / r2) * (PPG_PI / 4.0f); }
-    float s, c; sincosf(phi, &s, &c);
+    float s, c; sincosf_bounded(phi, &s, &c);                                  // |r1 / r2| <= 1: |phi| <= 3 pi / 4
     const float px = r * c, py = r * s;
     float z = sqrtf(fmaxf(0.0f, 1.0f - px * px - py * py));
     if (z == 0.f) z = 1e-10f;
@@ -1140,7 +1153,7 @@ __device__ __forceinline__ float3 canonical_to_dir(float2 p) {
     const float cosTheta = 2.f * p.x - 1.f;
     const float phi = 2.f * PPG_PI * p.y;
     const float sinTheta = sqrtf(1.f - cosTheta * cosTheta);
-    float s, c; sincosf(phi, &s, &c);
+    float s, c; sincosf_bounded(phi, &s, &c);                                  // p.y in [0, 1]
     return f3(sinTheta * c, sinTheta * s, cosTheta);
 }
 

@@ -1050,7 +1050,9 @@ static int ppg_set_scene_impl(ppg_integrator *h, const ppg_scene_desc *s) {
     }
     v.nTris = nt; v.nBvhNodes = (uint32_t) nBvh; v.nBsdfs = s->n_bsdfs; v.nEmitters = std::max<uint32_t>(s->n_emitters, 1);
     const size_t sceneBytes = 16 * ((size_t) 3 * nt + 6 * nt + nt + 2 * nBvh + PPG_BSDF_F4 * s->n_bsdfs + v.nEmitters + 2 * std::max<uint32_t>(v.nGroups, 1));
-    h->sceneSmemBytes = sceneBytes <= 48 * 1024 ? (uint32_t) sceneBytes : 0u;   // small scenes (CBOX: ~9 KB) live in shared memory
+    // tiny scenes (CBOX: ~9 KB) live in shared memory.  Only those with coplanar groups: the staged bounce kernels test the groups and have no
+    // BVH walk, whose 512-byte stack would put every thread's frame in local memory.
+    h->sceneSmemBytes = sceneBytes <= 48 * 1024 && v.nGroups != 0u ? (uint32_t) sceneBytes : 0u;
     // camera (src/sensors/perspective.cpp:120-298; lookAt columns: left, up, dir, origin -- transform.cpp:191-214)
     const float *m = s->camera.to_world;
     Camera &c = h->cam;
@@ -1813,7 +1815,7 @@ __global__ void op_sample_kernel(const SampNode *pool, const uint32_t *first, co
         out[3 * i] = d.x; out[3 * i + 1] = d.y; out[3 * i + 2] = d.z;
     }
 }
-__global__ void op_record_kernel(TreeView T, const uint32_t *rt, const float *rd, const float *rrad, const float *rpdf, const float *rw, size_t n, int filter) {
+__global__ void op_record_kernel(const __grid_constant__ TreeView T, const uint32_t *rt, const float *rd, const float *rrad, const float *rpdf, const float *rw, size_t n, int filter) {
     const size_t nPad = (n + 31) / 32 * 32;
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < nPad; i += (size_t) gridDim.x * blockDim.x) {
         const bool ok = i < n;
@@ -1835,7 +1837,7 @@ __global__ void op_lookup_kernel(const uint2 *snodes, const uint32_t *table, flo
     }
 }
 // Scene::sampleAttenuatedEmitterDirect at caller-supplied reference points, exactly as the bounce kernel's light-sampling block calls it
-__global__ void op_emitter_sample_kernel(SceneView scene, const float *ref, const float *refN, const float *smp, int maxInteractions, size_t n,
+__global__ void op_emitter_sample_kernel(const __grid_constant__ SceneView scene, const float *ref, const float *refN, const float *smp, int maxInteractions, size_t n,
                                          float *dOut, float *valueOut, float *pdfOut, float *distOut) {
     const SceneAccess<false> sc(scene);
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
@@ -1849,7 +1851,7 @@ __global__ void op_emitter_sample_kernel(SceneView scene, const float *ref, cons
         pdfOut[i] = ds.pdf; distOut[i] = dist;
     }
 }
-__global__ void op_env_pdf_kernel(SceneView scene, const float *dir, size_t n, float *pdfOut, float *valueOut) {
+__global__ void op_env_pdf_kernel(const __grid_constant__ SceneView scene, const float *dir, size_t n, float *pdfOut, float *valueOut) {
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
         const float3 d = f3(dir[3 * i], dir[3 * i + 1], dir[3 * i + 2]);
         pdfOut[i] = pdf_emitter_direct<true>(scene, PPG_ENV_EMITTER, f3(0, 0, 0), f3(0, 0, 0), d, f3(0, 0, 0), 0.f);

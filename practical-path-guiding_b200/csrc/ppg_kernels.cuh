@@ -66,7 +66,7 @@ __device__ __forceinline__ void record_into_leaf(const CommitParams &C, uint32_t
 }
 
 template <int RECORD>
-__global__ void __launch_bounds__(PPG_BLOCK) commit_kernel(const CommitParams P) {
+__global__ void __launch_bounds__(PPG_BLOCK) commit_kernel(const __grid_constant__ CommitParams P) {
     const bool neeSlab = blockIdx.y >= P.nSlabs;
     const uint32_t k = neeSlab ? blockIdx.y - P.nSlabs : blockIdx.y;
     const uint32_t n = P.liveCounts[k];
@@ -243,7 +243,7 @@ struct MaintParams {
 // a leaf splits while its building weight exceeds the threshold (GP:953-955), both children inherit the parent's
 // leaf record (shared sampling tree, Adam state) with half the building weight (GP:876-895).  Children are allocated
 // with a block prefix sum, so node numbering is deterministic (required for identical replicas across ranks).
-__global__ void __launch_bounds__(1024) stree_refine_kernel(MaintParams M, float threshold, uint32_t *overflow) {
+__global__ void __launch_bounds__(1024) stree_refine_kernel(const __grid_constant__ MaintParams M, float threshold, uint32_t *overflow) {
     __shared__ uint32_t sScan[1024];
     __shared__ uint32_t sBase, sBegin, sEnd, sAny;
     if (threadIdx.x == 0) { sBegin = 0; sEnd = *M.nNodes; }
@@ -318,7 +318,7 @@ __global__ void stree_table_kernel(const uint2 *snodes, uint32_t *table) {
 // the reference's stack discipline so that node numbering is identical to the reference's.
 // FILL == false: count nodes only (-> buildCount, buildDepth).  FILL == true: write the topology at buildBase and zero sums.
 template <bool FILL>
-__global__ void __launch_bounds__(128) dtree_reset_kernel(MaintParams M, const uint32_t *buildBase, int newMaxDepth, float subdivisionThreshold) {
+__global__ void __launch_bounds__(128) dtree_reset_kernel(const __grid_constant__ MaintParams M, const uint32_t *buildBase, int newMaxDepth, float subdivisionThreshold) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t leaf = blockIdx.x * blockDim.x + threadIdx.x; leaf < nNodes; leaf += gridDim.x * blockDim.x) {
         if (M.snodes[leaf].x != 0u) { if (!FILL) M.buildCount[leaf] = 0; continue; }
@@ -361,7 +361,7 @@ __global__ void __launch_bounds__(128) dtree_reset_kernel(MaintParams M, const u
 
 // DTree::build (GP:520-533, 346-366) + "sampling = building" (GP:610-613), one thread per S-tree leaf.
 // Children have larger indices than their parent (reset appends), so one reverse sweep equals the recursion.
-__global__ void __launch_bounds__(128) dtree_build_kernel(MaintParams M, const uint32_t *buildBase) {
+__global__ void __launch_bounds__(128) dtree_build_kernel(const __grid_constant__ MaintParams M, const uint32_t *buildBase) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t leaf = blockIdx.x * blockDim.x + threadIdx.x; leaf < nNodes; leaf += gridDim.x * blockDim.x) {
         if (M.snodes[leaf].x != 0u) continue;
@@ -394,7 +394,7 @@ __global__ void __launch_bounds__(128) dtree_build_kernel(MaintParams M, const u
 }
 
 // after reset: point every leaf at its new building tree and zero the building statistical weight (GP:457)
-__global__ void leaf_after_reset_kernel(MaintParams M, const uint32_t *buildBase) {
+__global__ void leaf_after_reset_kernel(const __grid_constant__ MaintParams M, const uint32_t *buildBase) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {
         float4 la = M.leafA[n]; la.y = __uint_as_float(buildBase[n]); M.leafA[n] = la;
@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(256) adam_scatter_kernel(const float4 *recA, c
 // chain runs; every lane then walks the chain redundantly on values handed around with shuffles (no divergence, no dependent global load in the
 // chain).  The first version (one THREAD per leaf, a dependent 24-byte fetch per record) spent ~0.3 us per record: 310 of 1000 ms on SPACESHIP
 // 640x360, where the hottest leaf of an iteration holds > 100 000 records.
-__global__ void __launch_bounds__(128) adam_seq_kernel(MaintParams M, const float4 *recA, const float2 *recB, const uint32_t *offset, uint32_t *count,
+__global__ void __launch_bounds__(128) adam_seq_kernel(const __grid_constant__ MaintParams M, const float4 *recA, const float2 *recB, const uint32_t *offset, uint32_t *count,
                                                        uint32_t *cursor, float ratioPower) {
     const uint32_t nNodes = *M.nNodes;
     const uint32_t lane = threadIdx.x & 31u, warpsPerGrid = (gridDim.x * blockDim.x) >> 5;
@@ -537,7 +537,7 @@ __global__ void __launch_bounds__(128) adam_seq_kernel(MaintParams M, const floa
 // N > 1 ranks: every rank replays its own records from the common state; the replicas are then merged.  The exchange buffer holds the SUM over
 // ranks of [iter - iterBefore | m1 | m2 | variable | batchAcc | batchGrad] (6 arrays of nNodes floats).  Step counts add up, moments and the
 // variable are averaged, and the batch accumulators add up RELATIVE to the common start (each rank's value contains the carried-over part once).
-__global__ void adam_pack_kernel(MaintParams M, float *out6, float *before3, const float *unused, int stage) {
+__global__ void adam_pack_kernel(const __grid_constant__ MaintParams M, float *out6, float *before3, const float *unused, int stage) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {
         const float *st = M.adam + 6 * (size_t) n;
@@ -547,7 +547,7 @@ __global__ void adam_pack_kernel(MaintParams M, float *out6, float *before3, con
         out6[4 * (size_t) nNodes + n] = st[4]; out6[5 * (size_t) nNodes + n] = st[5];
     }
 }
-__global__ void adam_merge_kernel(MaintParams M, const float *sum6, const float *before3, float invWorld, float worldMinus1) {
+__global__ void adam_merge_kernel(const __grid_constant__ MaintParams M, const float *sum6, const float *before3, float invWorld, float worldMinus1) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {
         float *st = M.adam + 6 * (size_t) n;
@@ -564,7 +564,7 @@ struct TreeStats {
     uint32_t leaves, leavesWithNodes; int depthMin, depthMax; float meanMin, meanMax, weightMin, weightMax;
     unsigned long long nodesMin, nodesMax; double depthSum, meanSum, nodesSum, weightSum;
 };
-__global__ void __launch_bounds__(1024) tree_stats_kernel(MaintParams M, TreeStats *out) {
+__global__ void __launch_bounds__(1024) tree_stats_kernel(const __grid_constant__ MaintParams M, TreeStats *out) {
     const uint32_t nNodes = *M.nNodes;
     uint32_t leaves = 0, withNodes = 0; int dMin = 0x7fffffff, dMax = 0; float rMin = 3.4e38f, rMax = 0.f, wMin = 3.4e38f, wMax = 0.f;
     unsigned long long nMin = ~0ull, nMax = 0ull; double dSum = 0, rSum = 0, nSum = 0, wSum = 0;
@@ -610,7 +610,7 @@ __global__ void __launch_bounds__(1024) tree_stats_kernel(MaintParams M, TreeSta
 // How far did the sampling fractions move in the replay that just ended?  Sum over leaves of steps * |f_after - f_before| and of steps, in fixed
 // point (2^-20) so that the result does not depend on the summation order: every rank derives the size of its next sub-batch from it
 // (perform_render_passes), and all ranks must decide alike.  `before4`: [iter | batchAcc | batchGrad | theta] saved by adam_pack_kernel stage 0.
-__global__ void adam_progress_kernel(MaintParams M, const float *before4, unsigned long long *out2) {
+__global__ void adam_progress_kernel(const __grid_constant__ MaintParams M, const float *before4, unsigned long long *out2) {
     const uint32_t nNodes = *M.nNodes;
     unsigned long long moved = 0, steps = 0;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {

@@ -29,7 +29,7 @@ namespace ppg {
 #endif
 
 template <bool FIRST, bool SPHERES>
-__global__ void __launch_bounds__(PPG_TRACE_BLOCK, PPG_TRACE_MIN_BLOCKS) trace_kernel(const RenderParams P) {
+__global__ void __launch_bounds__(PPG_TRACE_BLOCK, PPG_TRACE_MIN_BLOCKS) trace_kernel(const __grid_constant__ RenderParams P) {
     const SceneAccess<false> A_(P.scene);
     const SceneView &sc = P.scene;
     const uint32_t nIn = FIRST ? P.nPaths : *P.liveIn;
