@@ -308,7 +308,8 @@ int ppg_abi_version(void);
 int ppg_create(const ppg_params *params, int device, ppg_integrator **out);
 void ppg_destroy(ppg_integrator *h);
 
-/* Upload the scene (builds the BVH on the host, copies everything to HBM). */
+/* Upload the scene (builds the BVH on the host, copies everything to HBM).  The whole description is validated before
+ * anything is uploaded: a rejected scene leaves the previous one in place; a CUDA error during the upload leaves none. */
 int ppg_set_scene(ppg_integrator *h, const ppg_scene_desc *scene);
 
 /* Tile sharding (SURVEY 8e): this process renders only its share of the 32x32

@@ -69,9 +69,10 @@ class GuidedPathTracer:
             pass
 
     def set_scene(self, scene: SceneDesc):
-        self._scene_arrays = capi.SceneArrays(scene)
+        arrays = capi.SceneArrays(scene)
+        _check(self.lib, self.lib.ppg_set_scene(self._h, C.byref(arrays.desc)))
+        self._scene_arrays = arrays
         self.W, self.H = scene.film_width, scene.film_height
-        _check(self.lib, self.lib.ppg_set_scene(self._h, C.byref(self._scene_arrays.desc)))
         return self
 
     def set_shard(self, rank: int, world_size: int):

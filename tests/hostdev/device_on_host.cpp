@@ -1,12 +1,42 @@
 // TEST INFRASTRUCTURE -- C entry points over the product's CUDA device functions compiled for the host (see cuda_host_shim.h); same shape as oracle/microfacet_ref/wrapper.h.
+// Scenes are packed by the product's own pack_scene (ppg_scene.cpp, compiled into the same library) and the device code reads the packed arrays in place.
 #include "cuda_host_shim.h"
 #include "../../practical-path-guiding_b200/csrc/ppg_kernels.cuh"      // (includes ppg_device.cuh; the __global__ functions run here as plain loops of one thread)
+#include "../../practical-path-guiding_b200/csrc/ppg_scene.h"
 #include "../../include/ppg.h"
 #include <cstddef>
+#include <string>
 #include <vector>
 using namespace ppg;
 static inline float3 v3(const float *p, size_t i) { return make_float3(p[3 * i], p[3 * i + 1], p[3 * i + 2]); }
+// a packed scene with its SceneView bound to the packed arrays themselves
+struct HostScene { PackedScene p; SceneView v; EnvLight env; std::string error; };
+static int open_scene(const ppg_scene_desc &d, HostScene &hs) {
+    const int rc = pack_scene(d, hs.p, hs.error);
+    if (rc == PPG_OK) bind_scene(hs.p, [&](int i) { return hs.p.array(i).data; }, &hs.env, hs.v, hs.env);
+    return rc;
+}
+// the Bsdf load_bsdf reads from the record pack_scene writes for material `m`, in a one-triangle scene with the rough-transmittance tables `tables`
+static int packed_bsdf(const ppg_bsdf &m, const float *tables, uint32_t nTables, HostScene &hs, Bsdf &b) {
+    static const float pos[9] = {0, 0, 0, 1, 0, 0, 0, 1, 0};
+    static const uint32_t idx[3] = {0, 1, 2}, triShape[1] = {0};
+    ppg_shape sh{}; sh.n_triangles = 1; sh.bsdf = 0; sh.emitter = -1;
+    ppg_scene_desc d{}; d.n_vertices = 3; d.n_triangles = 1; d.n_shapes = 1; d.n_bsdfs = 1;
+    d.positions = pos; d.indices = idx; d.triangle_shape = triShape; d.shapes = &sh; d.bsdfs = &m; d.bsdf_tables = tables; d.n_bsdf_tables = nTables;
+    d.camera.film_width = d.camera.film_height = 1;
+    const int rc = open_scene(d, hs);
+    if (rc == PPG_OK) b = load_bsdf<true>(SceneAccess<false>(hs.v), 0);
+    return rc;
+}
 extern "C" {
+// pack_scene alone: its status, and its message in `error`
+int dev_pack_scene(const ppg_scene_desc *d, char *error, size_t error_len) {
+    HostScene hs; const int rc = pack_scene(*d, hs.p, hs.error);
+    snprintf(error, error_len, "%s", hs.error.c_str());
+    return rc;
+}
+void *dev_scene_open(const ppg_scene_desc *d) { HostScene *hs = new HostScene(); if (open_scene(*d, *hs) == PPG_OK) return hs; delete hs; return nullptr; }
+void dev_scene_close(void *hs) { delete (HostScene *) hs; }
 int dev_mf_eval(int type, float alpha, size_t n, const float *m, float *out) { for (size_t i = 0; i < n; ++i) out[i] = mf_eval(type, alpha, v3(m, i)); return 0; }
 int dev_mf_smith_g1(int type, float alpha, size_t n, const float *v, const float *m, float *out) { for (size_t i = 0; i < n; ++i) out[i] = mf_smithG1(type, alpha, v3(v, i), v3(m, i)); return 0; }
 int dev_mf_pdf(int type, float alpha, size_t n, const float *wi, const float *m, float *out) { for (size_t i = 0; i < n; ++i) out[i] = mf_pdfVisible(type, alpha, v3(wi, i), v3(m, i)); return 0; }
@@ -28,7 +58,7 @@ int dev_coordinate_system(size_t n, const float *a, float *b_out, float *c_out) 
     return 0;
 }
 int dev_square_to_cosine_hemisphere(size_t n, const float *s, float *out) { for (size_t i = 0; i < n; ++i) { const float3 v = square_to_cosine_hemisphere(s[2 * i], s[2 * i + 1]); out[3 * i] = v.x; out[3 * i + 1] = v.y; out[3 * i + 2] = v.z; } return 0; }
-// the kernels' triangle test on the accel rows ppg_set_scene packs: {n_u, n_v, n_d, bits(k)}, {a_u, a_v, b_nu, b_nv}, {c_nu, c_nv, -, -}
+// the kernels' triangle test on the accel rows pack_scene writes: {n_u, n_v, n_d, bits(k)}, {a_u, a_v, b_nu, b_nv}, {c_nu, c_nv, -, -}
 int dev_tri_intersect(size_t n, const int *k, const float *consts /* 9n, TriAccel order */, const float *o, const float *d, const float *mint, const float *maxt, unsigned char *hit_out, float *tuv_out) {
     for (size_t i = 0; i < n; ++i) {
         const float *c = consts + 9 * i;
@@ -39,32 +69,17 @@ int dev_tri_intersect(size_t n, const int *k, const float *consts /* 9n, TriAcce
     }
     return 0;
 }
-// ---- whole BSDF models: the device Bsdf record as load_bsdf() rebuilds it from the 28 floats ppg_set_scene packs per material (ppg_host.cu: "bsdf" table)
-static Bsdf make_bsdf(const ppg_bsdf &m, const float *tables) {
-    Bsdf b; b.refl = make_float3(m.reflectance[0], m.reflectance[1], m.reflectance[2]);
-    b.type = (uint32_t) m.type; b.flags = m.flags & 0xffffffu;
-    if (m.type == PPG_BSDF_NULL_BLACK) { b.refl = make_float3(0, 0, 0); b.type = PPG_BSDF_T_DIFFUSE; }
-    b.trans = b.etaRgb = b.k = b.specRefl = make_float3(0, 0, 0); b.eta = b.invEta = 1.f; b.alpha = 0.1f; b.distr = 1; b.fdrInt = b.ssw = 0.f; b.lut = nullptr;
-    b.opacity = make_float3(1, 1, 1); b.maskProb = 1.f; b.reflTex = b.bumpTex = 0u;
-    if (b.flags & PPG_BSDF_MASK) { b.opacity = make_float3(m.opacity[0], m.opacity[1], m.opacity[2]); b.maskProb = m.opacity[0] * 0.212671f + m.opacity[1] * 0.715160f + m.opacity[2] * 0.072169f; }
-    if (b.type != PPG_BSDF_T_DIFFUSE) {
-        b.trans = make_float3(m.specular_transmittance[0], m.specular_transmittance[1], m.specular_transmittance[2]); b.eta = m.eta[0];
-        b.etaRgb = make_float3(m.eta[0], m.eta[1], m.eta[2]); b.invEta = m.eta[0] != 0.f ? 1.0f / m.eta[0] : 0.f; b.k = make_float3(m.k[0], m.k[1], m.k[2]);
-        b.alpha = std::max(m.alpha, 1e-4f); b.distr = m.distribution == PPG_MICROFACET_BECKMANN ? 0 : 1;
-        if (b.type == PPG_BSDF_T_ROUGHPLASTIC || b.type == PPG_BSDF_T_PLASTIC) {
-            b.specRefl = make_float3(m.specular_reflectance[0], m.specular_reflectance[1], m.specular_reflectance[2]); b.fdrInt = m.fdr_int; b.ssw = m.specular_sampling_weight;
-            b.lut = tables ? tables + (size_t) std::max(m.table, 0) * PPG_BSDF_LUT : nullptr;
-        }
-    }
-    return b;
-}
-int dev_bsdf_eval_pdf(const ppg_bsdf *m, size_t n, const float *wi, const float *wo, float *eval_out, float *pdf_out, const float *tables) {
-    const Bsdf b = make_bsdf(*m, tables);
+// ---- whole BSDF models, as load_bsdf() reads them from the packed material record
+int dev_bsdf_eval_pdf(const ppg_bsdf *m, size_t n, const float *wi, const float *wo, float *eval_out, float *pdf_out, const float *tables, uint32_t n_tables) {
+    HostScene hs; Bsdf b;
+    if (const int rc = packed_bsdf(*m, tables, n_tables, hs, b)) return rc;
     for (size_t i = 0; i < n; ++i) { const float3 e = bsdf_eval(b, v3(wi, i), v3(wo, i)); eval_out[3 * i] = e.x; eval_out[3 * i + 1] = e.y; eval_out[3 * i + 2] = e.z; pdf_out[i] = bsdf_pdf(b, v3(wi, i), v3(wo, i)); }
     return 0;
 }
-int dev_bsdf_sample(const ppg_bsdf *m, size_t n, const float *wi, const float *sample, float *wo_out, float *weight_out, float *pdf_out, unsigned char *delta_out, const float *tables) {
-    const Bsdf b = make_bsdf(*m, tables);
+int dev_bsdf_sample(const ppg_bsdf *m, size_t n, const float *wi, const float *sample, float *wo_out, float *weight_out, float *pdf_out, unsigned char *delta_out,
+                    const float *tables, uint32_t n_tables) {
+    HostScene hs; Bsdf b;
+    if (const int rc = packed_bsdf(*m, tables, n_tables, hs, b)) return rc;
     for (size_t i = 0; i < n; ++i) {
         float3 wo = make_float3(0, 0, 0); float eta = 1.f, pdf = 0.f; bool delta = false, isNull = false;
         Pcg32 extra; extra.seed(splitmix64(i), i);                      // like ppgo_bsdf_sample: the model's own draws from the path sampler (roughdielectric)
@@ -74,25 +89,21 @@ int dev_bsdf_sample(const ppg_bsdf *m, size_t n, const float *wi, const float *s
     }
     return 0;
 }
-// bitmap textures: one ppg_texture packed the way ppg_set_scene packs it (uint2 {r | g << 16, b} per texel, two float4 of meta), then tex_eval / tex_gradient_lum
-int dev_texture_eval(const ppg_texture *t, const uint16_t *texels /* the whole texel array of the scene */, size_t n, const float *uv, float *rgb_out, float *grad_out) {
-    const size_t nTexels = (size_t) t->width * t->height;
-    std::vector<uint2> tex(nTexels);
-    const uint16_t *src = texels + t->first_texel;
-    for (size_t i = 0; i < nTexels; ++i) {
-        const uint16_t r = src[i * t->channels], g = t->channels == 3 ? src[i * t->channels + 1] : r, b = t->channels == 3 ? src[i * t->channels + 2] : r;
-        tex[i] = make_uint2((uint32_t) r | ((uint32_t) g << 16), (uint32_t) b);
-    }
-    float4 meta[2];
-    const uint32_t wr = t->wrap_u | (t->wrap_v << 8);
-    meta[0] = make_float4(__uint_as_float(t->width), __uint_as_float(t->height), __uint_as_float(wr), __uint_as_float(0u));
-    meta[1] = make_float4(t->uv_scale[0], t->uv_scale[1], t->uv_offset[0], t->uv_offset[1]);
-    SceneView sc; memset(&sc, 0, sizeof(sc)); sc.texMeta = meta; sc.texels = tex.data(); sc.nTextures = 1;
+// bitmap textures: tex_eval / tex_gradient_lum of texture `k` of a packed scene
+int dev_texture_eval(const void *scene, uint32_t k, size_t n, const float *uv, float *rgb_out, float *grad_out) {
+    const SceneView &sc = ((const HostScene *) scene)->v;
     for (size_t i = 0; i < n; ++i) {
         const float2 q = make_float2(uv[2 * i], uv[2 * i + 1]);
-        const float3 c = tex_eval(sc, 0u, q); const float2 g = tex_gradient_lum(sc, 0u, q);
+        const float3 c = tex_eval(sc, k, q); const float2 g = tex_gradient_lum(sc, k, q);
         rgb_out[3 * i] = c.x; rgb_out[3 * i + 1] = c.y; rgb_out[3 * i + 2] = c.z; grad_out[2 * i] = g.x; grad_out[2 * i + 1] = g.y;
     }
+    return 0;
+}
+// the emitter-list table the host builds from `n_entries` weights: running float sum, then normalize_cdf (n_entries + 1 values)
+int dev_emitter_cdf(size_t n_entries, const float *weights, float *cdf_out) {
+    cdf_out[0] = 0.f;
+    for (size_t i = 0; i < n_entries; ++i) cdf_out[i + 1] = cdf_out[i] + weights[i];
+    normalize_cdf(cdf_out, n_entries);
     return 0;
 }
 // cdf_sample + the sample reuse of the device's sample_emitter_direct, on a normalised cdf (n_entries + 1 values) the host built
@@ -133,6 +144,54 @@ int dev_dtree(const float *sums, const uint16_t *children, size_t n_nodes, const
         ReplayRng r{rnd + rnd_stride * i, (uint32_t) rnd_stride, 0u};
         const float3 d = canonical_to_dir(dtree_sample(pool.data() + tree_first[t], mean > 0.f, r));
         dir_out[3 * i] = d.x; dir_out[3 * i + 1] = d.y; dir_out[3 * i + 2] = d.z;
+    }
+    return 0;
+}
+// ---- packed scenes: nearest hit, light sampling, environment emitter
+// bvh_intersect (coplanar groups or BVH walk, whichever the packing chose), and the brute-force minimum of tri_intersect over every packed accel row
+// (ties to the lower original triangle index).  t_out / prim_out: 2 per ray {bvh_intersect, brute force}; prim 0xFFFFFFFF = miss.
+int dev_closest_hit(const void *scene, size_t n, const float *o, const float *d, float mint, float maxt, float *t_out, uint32_t *prim_out) {
+    const SceneView &sc = ((const HostScene *) scene)->v;
+    const SceneAccess<false> acc(sc);
+    for (size_t i = 0; i < n; ++i) {
+        Hit h; h.t = 0.f;
+        const bool found = bvh_intersect<true>(acc, v3(o, i), v3(d, i), mint, maxt, h);
+        t_out[2 * i] = found ? h.t : 0.f; prim_out[2 * i] = found ? h.prim : 0xFFFFFFFFu;
+        float bt = __int_as_float(0x7f800000); uint32_t bp = 0xFFFFFFFFu;
+        for (uint32_t s = 0; s < sc.nTris; ++s) {
+            float u, v, t;
+            const float4 A = sc.accel[3 * s], B = sc.accel[3 * s + 1], C = sc.accel[3 * s + 2];
+            if (!tri_intersect(A, B, C, v3(o, i), v3(d, i), mint, maxt, u, v, t)) continue;
+            const uint32_t prim = __float_as_uint(C.z);
+            if (t < bt || (t == bt && prim < bp)) { bt = t; bp = prim; }
+        }
+        t_out[2 * i + 1] = bp != 0xFFFFFFFFu ? bt : 0.f; prim_out[2 * i + 1] = bp;
+    }
+    return 0;
+}
+// the body of op_emitter_sample_kernel (ppg_host.cu): Scene::sampleAttenuatedEmitterDirect at caller-supplied reference points
+int dev_emitter_sample_direct(const void *scene, size_t n, const float *ref, const float *refN, const float *smp, int maxInteractions,
+                              float *dOut, float *valueOut, float *pdfOut, float *distOut) {
+    const SceneAccess<false> sc(((const HostScene *) scene)->v);
+    for (size_t i = 0; i < n; ++i) {
+        const float3 p = v3(ref, i), rn = v3(refN, i);
+        DirectSample ds; ds.value = make_float3(0, 0, 0); ds.d = make_float3(0, 0, 0); ds.pdf = 0.f; float dist = 0.f;
+        const bool ok = sample_emitter_direct<true>(sc, p, rn, smp[2 * i], smp[2 * i + 1], ds, dist);
+        if (ok) ds.value = ds.value * eval_transmittance(sc, p, ds.d, dist, maxInteractions);
+        else { ds.value = make_float3(0, 0, 0); ds.pdf = 0.f; dist = 0.f; }
+        dOut[3 * i] = ds.d.x; dOut[3 * i + 1] = ds.d.y; dOut[3 * i + 2] = ds.d.z;
+        valueOut[3 * i] = ds.value.x; valueOut[3 * i + 1] = ds.value.y; valueOut[3 * i + 2] = ds.value.z;
+        pdfOut[i] = ds.pdf; distOut[i] = dist;
+    }
+    return 0;
+}
+// the body of op_env_pdf_kernel (ppg_host.cu): the environment emitter's pdfEmitterDirect and radiance for world directions
+int dev_env_pdf(const void *scene, size_t n, const float *dir, float *pdfOut, float *valueOut) {
+    const SceneView &sc = ((const HostScene *) scene)->v;
+    for (size_t i = 0; i < n; ++i) {
+        const float3 d = v3(dir, i);
+        pdfOut[i] = pdf_emitter_direct<true>(sc, PPG_ENV_EMITTER, make_float3(0, 0, 0), make_float3(0, 0, 0), d, make_float3(0, 0, 0), 0.f);
+        const float3 v = env_eval(sc, d); valueOut[3 * i] = v.x; valueOut[3 * i + 1] = v.y; valueOut[3 * i + 2] = v.z;
     }
     return 0;
 }

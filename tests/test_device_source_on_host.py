@@ -2,7 +2,9 @@
 float3 / float4, the intrinsics get host meanings) and compared, function by function and bit for bit, with the reference's own code compiled verbatim
 (oracle/_ref/libmicrofacet_ref.so) -- or with the oracle's restatement where the reference tree was absent at build time.  The kernels are built with -fmad=false
 -prec-div=true -prec-sqrt=true, this harness with -ffp-contract=off: +, -, *, / and sqrt round identically; only the libm calls are the host's here and the
-device's on the GPU (their ulps are what the `-m gpu` parity tests allow for).  So: reference source == oracle == the source the kernels are compiled from."""
+device's on the GPU (their ulps are what the `-m gpu` parity tests allow for).  So: reference source == oracle == the source the kernels are compiled from.
+The scenes the device code reads here are packed by the library's own host module (csrc/ppg_scene.cpp, compiled into the harness): the same bytes
+ppg_set_scene uploads, so the packing is part of the chain."""
 import ctypes as C
 import os
 import shutil
@@ -23,10 +25,30 @@ f32p = C.POINTER(C.c_float)
 def dev(tmp_path_factory):
     so = str(tmp_path_factory.mktemp("hostdev") / "libdevice_on_host.so")
     cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I" + CUDA_INC, "-D__device__=", "-D__host__=", "-D__global__=", "-D__shared__=",
-           "-D__forceinline__=inline", "-D__noinline__=", "-D__launch_bounds__(...)=", "-Wno-unused-function", os.path.join(ROOT, "tests", "hostdev", "device_on_host.cpp"), "-o", so]
+           "-D__forceinline__=inline", "-D__noinline__=", "-D__launch_bounds__(...)=", "-Wno-unused-function", os.path.join(ROOT, "tests", "hostdev", "device_on_host.cpp"),
+           os.path.join(ROOT, "practical-path-guiding_b200", "csrc", "ppg_scene.cpp"), "-o", so]
     r = subprocess.run(cmd, capture_output=True, text=True)
     assert r.returncode == 0, r.stderr[-3000:]
-    return C.CDLL(so)
+    lib = C.CDLL(so)
+    lib.dev_scene_open.restype = C.c_void_p; lib.dev_scene_open.argtypes = [C.c_void_p]
+    lib.dev_scene_close.restype = None; lib.dev_scene_close.argtypes = [C.c_void_p]
+    return lib
+
+
+class _Packed:
+    """A scene packed by pack_scene inside the harness, its SceneView bound to the packed arrays (a context manager)."""
+
+    def __init__(self, dev, scene):
+        from ppg_b200 import capi
+        self.dev, self.arrays = dev, capi.SceneArrays(scene)
+        self.h = dev.dev_scene_open(C.addressof(self.arrays.desc))
+        assert self.h, "pack_scene rejected the scene"
+
+    def __enter__(self):
+        return self.h
+
+    def __exit__(self, *exc):
+        self.dev.dev_scene_close(self.h)
 
 
 def _truth():
@@ -99,7 +121,7 @@ def test_device_helper_sources_equal_the_reference(dev):
 
 
 def test_device_triangle_test_and_transmittance_sources_equal_the_reference(dev):
-    """tri_intersect on the accel rows ppg_set_scene packs, fed with the reference's own TriAccel constants: same hit decision, same (t, u, v) as TriAccel::rayIntersect."""
+    """tri_intersect on the accel rows pack_scene writes, fed with the reference's own TriAccel constants: same hit decision, same (t, u, v) as TriAccel::rayIntersect."""
     truth = C.CDLL(O.MFREF_SO) if os.path.exists(O.MFREF_SO) else O.load("port"); name = "mfref_triaccel" if os.path.exists(O.MFREF_SO) else "ppgo_triaccel"
     rng = np.random.default_rng(5); n = 200000
     A = rng.normal(size=(n, 3)).astype(np.float32) * 10; B = A + rng.normal(size=(n, 3)).astype(np.float32); Cc = A + rng.normal(size=(n, 3)).astype(np.float32)
@@ -172,22 +194,25 @@ MATERIALS = list(SIMPLE) + list(ROUGHPLASTICS) + ["plastic nonlinear", "plastic 
 def test_device_bsdf_sources_equal_the_oracle(dev, name):
     """bsdf_eval / bsdf_pdf / bsdf_sample of csrc/ppg_device.cuh (host-compiled) against the oracle's restatement of the same Mitsuba models, on the same directions and
     random numbers: every value bit for bit -- eval and pdf on 10^5 direction pairs over the whole sphere (both sides of the surface), sampling on 10^5 (wi, u) pairs
-    incl. the model's own extra draw (roughdielectric) and the delta / null lobes."""
+    incl. the model's own extra draw (roughdielectric) and the delta / null lobes.  The device side is the material as load_bsdf reads it from the record
+    pack_scene writes for it (a one-triangle scene with the material's tables)."""
     b, tables = _material(name)
+    nt = tables.size // 100 if tables is not None else 0
     rng = np.random.default_rng(MATERIALS.index(name)); n = 100000
     wi, wo = _dirs(rng, n, False), _dirs(rng, n, False)
     wi[:200, 2] = np.abs(wi[:200, 2]) * 1e-3; wi[:200] /= np.linalg.norm(wi[:200], axis=1, keepdims=True)         # grazing incidence
     wo[200:1200] = wi[200:1200] * [-1, -1, 1]                                                                    # the mirror direction (delta lobes evaluate to 0 without the discrete measure)
     tp = tables.ctypes.data_as(f32p) if tables is not None else None
     ev = np.zeros((n, 3), np.float32); pd = np.zeros(n, np.float32)
-    dev.dev_bsdf_eval_pdf.argtypes = [C.POINTER(type(b)), C.c_size_t, f32p, f32p, f32p, f32p, f32p]
-    dev.dev_bsdf_eval_pdf(C.byref(b), n, wi.ctypes.data_as(f32p), wo.ctypes.data_as(f32p), ev.ctypes.data_as(f32p), pd.ctypes.data_as(f32p), tp)
+    dev.dev_bsdf_eval_pdf.argtypes = [C.POINTER(type(b)), C.c_size_t, f32p, f32p, f32p, f32p, f32p, C.c_uint32]
+    assert dev.dev_bsdf_eval_pdf(C.byref(b), n, wi.ctypes.data_as(f32p), wo.ctypes.data_as(f32p), ev.ctypes.data_as(f32p), pd.ctypes.data_as(f32p), tp, nt) == 0
     ev0, pd0 = O.bsdf_eval_pdf(b, wi, wo, tables=tables)
     assert np.array_equal(ev.view(np.uint32), ev0.view(np.uint32)) and np.array_equal(pd.view(np.uint32), pd0.view(np.uint32))
     smp = rng.random((n, 2), dtype=np.float32)
     so = np.zeros((n, 3), np.float32); sw = np.zeros((n, 3), np.float32); sp = np.zeros(n, np.float32); sd = np.zeros(n, np.uint8)
-    dev.dev_bsdf_sample.argtypes = [C.POINTER(type(b)), C.c_size_t, f32p, f32p, f32p, f32p, f32p, C.POINTER(C.c_ubyte), f32p]
-    dev.dev_bsdf_sample(C.byref(b), n, wi.ctypes.data_as(f32p), smp.ctypes.data_as(f32p), so.ctypes.data_as(f32p), sw.ctypes.data_as(f32p), sp.ctypes.data_as(f32p), sd.ctypes.data_as(C.POINTER(C.c_ubyte)), tp)
+    dev.dev_bsdf_sample.argtypes = [C.POINTER(type(b)), C.c_size_t, f32p, f32p, f32p, f32p, f32p, C.POINTER(C.c_ubyte), f32p, C.c_uint32]
+    assert dev.dev_bsdf_sample(C.byref(b), n, wi.ctypes.data_as(f32p), smp.ctypes.data_as(f32p), so.ctypes.data_as(f32p), sw.ctypes.data_as(f32p), sp.ctypes.data_as(f32p),
+                               sd.ctypes.data_as(C.POINTER(C.c_ubyte)), tp, nt) == 0
     so0, sw0, sp0, sd0 = O.bsdf_sample(b, wi, smp, tables=tables)
     lit = (sw0 != 0).any(axis=1)                                                    # a failed sample carries weight 0; its wo is unspecified on both sides
     assert np.array_equal(lit, (sw != 0).any(axis=1)) and (lit.mean() > 0.2 or b.type == 1)
@@ -197,31 +222,30 @@ def test_device_bsdf_sources_equal_the_oracle(dev, name):
 
 def test_device_texture_source_equals_the_oracle(dev):
     """tex_eval (BitmapTexture::eval -> TMIPMap::evalBilinear, level 0) and tex_gradient_lum (evalGradientBilinear -> the luminances BumpMap::getFrame uses) of the
-    device source on the textures of the cbox-textured fixture (RGB and one-channel, repeat / clamp / mirror wrapping, uv scale and offset), packed the way
-    ppg_set_scene packs them, against the oracle's texture code at 10^5 texture coordinates reaching far outside [0, 1]^2: bit for bit."""
+    device source on the textures of the cbox-textured fixture (RGB and one-channel, repeat / clamp / mirror wrapping, uv scale and offset), read from the
+    whole scene as pack_scene packs it, against the oracle's texture code at 10^5 texture coordinates reaching far outside [0, 1]^2: bit for bit."""
     from common import load_fixture_scene
-    from ppg_b200 import capi
     sc = load_fixture_scene("cbox-textured")
     o = O.Oracle(O.params_from_xml(sc.integrator), sc, kind="port")
     lib = O.load("port"); lib.ppgo_texture_eval.argtypes = [C.c_void_p, C.c_uint32, C.c_size_t, f32p, f32p, f32p]
     arrays = o.scene_arrays
     rng = np.random.default_rng(17); n = 100000
     uv = (rng.random((n, 2)) * 6 - 2.5).astype(np.float32); uv[:4] = [[0, 0], [1, 1], [0.5, 0.5], [np.nan, 0.3]]
-    dev.dev_texture_eval.argtypes = [C.POINTER(capi.PpgTexture), C.POINTER(C.c_uint16), C.c_size_t, f32p, f32p, f32p]
+    dev.dev_texture_eval.argtypes = [C.c_void_p, C.c_uint32, C.c_size_t, f32p, f32p, f32p]
     assert len(sc.textures) == 3
-    for k in range(len(sc.textures)):
-        a = np.zeros((n, 3), np.float32); ga = np.zeros((n, 2), np.float32); b = np.zeros((n, 3), np.float32); gb = np.zeros((n, 2), np.float32)
-        assert lib.ppgo_texture_eval(o.h, k, n, uv.ctypes.data_as(f32p), a.ctypes.data_as(f32p), ga.ctypes.data_as(f32p)) == 0
-        t = capi.PpgTexture.from_buffer_copy(np.ascontiguousarray(sc.textures[k:k + 1]).tobytes())
-        texels = np.ascontiguousarray(sc.texels, np.uint16)
-        dev.dev_texture_eval(C.byref(t), texels.ctypes.data_as(C.POINTER(C.c_uint16)), n, uv.ctypes.data_as(f32p), b.ctypes.data_as(f32p), gb.ctypes.data_as(f32p))
-        assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) and np.array_equal(ga.view(np.uint32), gb.view(np.uint32)), k
-        assert np.abs(a[4:]).max() > 0.1 and np.abs(ga[4:]).max() > 0
+    with _Packed(dev, sc) as h:
+        for k in range(len(sc.textures)):
+            a = np.zeros((n, 3), np.float32); ga = np.zeros((n, 2), np.float32); b = np.zeros((n, 3), np.float32); gb = np.zeros((n, 2), np.float32)
+            assert lib.ppgo_texture_eval(o.h, k, n, uv.ctypes.data_as(f32p), a.ctypes.data_as(f32p), ga.ctypes.data_as(f32p)) == 0
+            assert dev.dev_texture_eval(h, k, n, uv.ctypes.data_as(f32p), b.ctypes.data_as(f32p), gb.ctypes.data_as(f32p)) == 0
+            assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) and np.array_equal(ga.view(np.uint32), gb.view(np.uint32)), k
+            assert np.abs(a[4:]).max() > 0.1 and np.abs(ga[4:]).max() > 0
 
 
 def test_device_discrete_sampling_source_equals_the_reference(dev):
-    """cdf_sample + the sample reuse of the device's sample_emitter_direct on the normalised table ppg_set_scene uploads, against DiscreteDistribution::sampleReuse of the
-    reference compiled verbatim (or the oracle's, bit-equal to it): index and reused sample bit for bit, zero-weight entries skipped the same way."""
+    """cdf_sample + the sample reuse of the device's sample_emitter_direct on the normalised table pack_scene builds (running sum, normalize_cdf), against
+    DiscreteDistribution::sampleReuse of the reference compiled verbatim (or the oracle's, bit-equal to it): table, index and reused sample bit for bit,
+    zero-weight entries skipped the same way."""
     have_ref = os.path.exists(O.MFREF_SO)
     truth = C.CDLL(O.MFREF_SO) if have_ref else O.load("port"); name = "mfref_discrete" if have_ref else "ppgo_discrete"
     u32p = C.POINTER(C.c_uint32)
@@ -236,11 +260,9 @@ def test_device_discrete_sampling_source_equals_the_reference(dev):
         pdf = np.zeros(ne, np.float32); s = C.c_float(); idx = np.zeros(n, np.uint32); reuse = np.zeros(n, np.float32)
         fn = getattr(truth, name); fn.argtypes = [C.c_size_t, f32p, C.c_size_t, f32p, f32p, C.POINTER(C.c_float), u32p, f32p]
         fn(ne, w.ctypes.data_as(f32p), n, smp.ctypes.data_as(f32p), pdf.ctypes.data_as(f32p), C.byref(s), idx.ctypes.data_as(u32p), reuse.ctypes.data_as(f32p))
-        # the table as the host builds it (ppg_host.cu, emitter tables: cumulative sum, x 1/sum, last entry = 1): DiscreteDistribution::normalize
         cdf = np.zeros(ne + 1, np.float32)
-        for i in range(ne):
-            cdf[i + 1] = np.float32(cdf[i] + w[i])
-        nrm = np.float32(1.0) / cdf[-1]; cdf[1:] = cdf[1:] * nrm; cdf[-1] = 1.0
+        dev.dev_emitter_cdf.argtypes = [C.c_size_t, f32p, f32p]
+        dev.dev_emitter_cdf(ne, w.ctypes.data_as(f32p), cdf.ctypes.data_as(f32p))
         assert np.array_equal(np.diff(cdf), pdf) or np.allclose(np.diff(cdf), pdf, rtol=0, atol=0)
         idx2 = np.zeros(n, np.uint32); reuse2 = np.zeros(n, np.float32)
         dev.dev_discrete.argtypes = [C.c_size_t, f32p, C.c_size_t, f32p, u32p, f32p]
@@ -278,3 +300,142 @@ def test_device_sdtree_sources_against_the_reference_trees(dev):
     ref_pdf = o.pdf(ql, d); ref_dir = o.sample(ql, rnd)
     assert np.allclose(pdf, ref_pdf, rtol=2e-6, atol=1e-12) and np.abs(dirs - ref_dir).max() <= 2e-6
     assert (dirs == ref_dir).all(axis=1).mean() > 0.9                              # (mostly bit-equal: same libm here)
+
+
+def _bsdf_ints(a):
+    return a.bsdfs.view(np.int32)          # ppg_bsdf as 28 int32: type 0, flags 1, eta 8-10, table 21, reflectance_texture 25, bump_texture 26
+
+
+def _shape_of_textured_bsdf(a):
+    return int(np.nonzero(_bsdf_ints(a)[a.shapes[:, 2], 25] != 0)[0][0])
+
+
+def _sphere_on(a, shape, radius=1.0):
+    a.extra = np.zeros((1, 6), np.float32); a.extra[0, 3] = radius; a.extra.view(np.int32)[0, 4] = shape
+    a.desc.n_spheres = 1; a.desc.spheres = C.cast(a.extra.ctypes.data, type(a.desc.spheres))
+
+
+def _emitter_shape(a):
+    return int(np.nonzero(a.shapes[:, 3] >= 0)[0][0])
+
+
+INVALID, UNSUPPORTED = -1, -6
+# (fixture, change to the description, expected status, part of the message); every validation path of pack_scene
+REJECTIONS = {
+    "no triangles": ("cbox", lambda a: setattr(a.desc, "n_triangles", 0), INVALID, "needs triangles"),
+    "emitters without radiance": ("cbox", lambda a: setattr(a.desc, "area_radiance", None), INVALID, "without its array"),
+    "film size 0": ("cbox", lambda a: setattr(a.desc.camera, "film_width", 0), INVALID, "film size"),
+    "film size 65536": ("cbox", lambda a: setattr(a.desc.camera, "film_height", 65536), INVALID, "film size"),
+    "triangle_shape out of range": ("cbox", lambda a: a.triangle_shape.__setitem__(3, len(a.shapes)), INVALID, "triangle_shape out of range"),
+    "vertex index out of range": ("cbox", lambda a: a.indices.__setitem__((5, 1), len(a.positions)), INVALID, "vertex index out of range"),
+    "shape bsdf out of range": ("cbox", lambda a: a.shapes.__setitem__((0, 2), len(a.bsdfs)), INVALID, "shape bsdf out of range"),
+    "shape emitter out of range": ("cbox", lambda a: a.shapes.__setitem__((0, 3), len(a.radiance)), INVALID, "shape emitter out of range"),
+    "unsupported bsdf": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, 0), 9), UNSUPPORTED, "hot-path scope"),
+    "mask around thindielectric": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, slice(0, 2)), (8, 4)), UNSUPPORTED, "mask around"),
+    "roughplastic without a table": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, 0), 5), INVALID, "rough-transmittance table"),
+    "roughplastic table out of range": ("cbox-plastic", lambda a: setattr(a.desc, "n_bsdf_tables", 0), INVALID, "rough-transmittance table"),
+    "dielectric without eta": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, 0), 2), INVALID, "eta > 0"),
+    "twosided dielectric": ("cbox", lambda a: (_bsdf_ints(a).__setitem__((0, slice(0, 2)), (2, 1)), a.bsdfs.__setitem__((0, 8), 1.5)), INVALID, "twosided cannot wrap"),
+    "texture index out of range": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, 25), 1), INVALID, "texture index out of range"),
+    "texture on a conductor": ("cbox-textured", lambda a: _bsdf_ints(a).__setitem__((int(a.shapes[_shape_of_textured_bsdf(a), 2]), 0), 3), UNSUPPORTED, "only the diffuse reflectance"),
+    "bumpmap without texture": ("cbox", lambda a: _bsdf_ints(a).__setitem__((0, 1), 8), INVALID, "displacement texture"),
+    "textures without texels": ("cbox-textured", lambda a: setattr(a.desc, "texels", None), INVALID, "without texel data"),
+    "texture of width 0": ("cbox-textured", lambda a: a.textures["width"].__setitem__(0, 0), INVALID, "bad size"),
+    "texture with 2 channels": ("cbox-textured", lambda a: a.textures["channels"].__setitem__(1, 2), INVALID, "bad size"),
+    "texture wrap mode 3": ("cbox-textured", lambda a: a.textures["wrap_v"].__setitem__(2, 3), INVALID, "bad size"),
+    "texel range out of bounds": ("cbox-textured", lambda a: setattr(a.desc, "n_texels", len(a.texels) - 1), INVALID, "texel range"),
+    "texture on a sphere": ("cbox-textured", lambda a: _sphere_on(a, _shape_of_textured_bsdf(a)), UNSUPPORTED, "analytic sphere"),
+    "envmap without texels": ("env", lambda a: setattr(a.desc.envmap, "texels", None), INVALID, "envmap without texel data"),
+    "black envmap": ("env", lambda a: a.env_texels.fill(0), INVALID, "completely black"),
+    "NaN in the envmap": ("env", lambda a: a.env_texels.__setitem__((3, 5, 1), 0x7E00), INVALID, "nan/inf"),
+    "singular world_to_env": ("env", lambda a: [a.desc.envmap.world_to_env.__setitem__(i, 0.0) for i in range(3)], INVALID, "singular world_to_env"),
+    "sphere of radius 0": ("spheres", lambda a: a.spheres.__setitem__((0, 3), 0.0), INVALID, "bad shape index or radius"),
+    "sphere without a shape": ("spheres", lambda a: a.spheres.view(np.int32).__setitem__((1, 4), -1), INVALID, "bad shape index or radius"),
+    "emitter triangle range out of bounds": ("cbox", lambda a: a.shapes.__setitem__((_emitter_shape(a), 1), len(a.indices) + 1), INVALID, "triangle range out of bounds"),
+    "2^32 texels": ("cbox-textured", lambda a: (a.textures["width"].__setitem__(0, 65536), a.textures["height"].__setitem__(0, 65536), a.textures["channels"].__setitem__(0, 1),
+                                                a.textures["first_texel"].__setitem__(0, 0), setattr(a.desc, "n_texels", 1 << 32)), UNSUPPORTED, "2^32 texels"),
+}
+
+
+def _fixture(name):
+    from common import load_cbox, load_fixture_scene
+    from ppg_b200 import builtin_scenes as B
+    if name == "cbox":
+        return load_cbox(32)
+    if name == "env":
+        return B.env_lit_scene(32)
+    if name == "spheres":
+        return B.cbox_with_analytic_spheres(load_cbox(32))
+    return load_fixture_scene(name, 32)
+
+
+@pytest.mark.parametrize("case", list(REJECTIONS))
+def test_pack_scene_rejects_malformed_scenes(dev, case):
+    """pack_scene validates the whole description before anything is uploaded: each malformed variant of a fixture scene gets its documented status and
+    message, and the unmodified fixture packs."""
+    from ppg_b200 import capi
+    fixture, change, code, message = REJECTIONS[case]
+    err = C.create_string_buffer(256)
+    dev.dev_pack_scene.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
+    a = capi.SceneArrays(_fixture(fixture))
+    assert dev.dev_pack_scene(C.addressof(a.desc), err, len(err)) == 0, err.value
+    change(a)
+    assert dev.dev_pack_scene(C.addressof(a.desc), err, len(err)) == code, err.value
+    assert message in err.value.decode(), err.value
+
+
+@pytest.mark.parametrize("scene", ["cbox", "torus"])
+def test_closest_hit_on_packed_scenes_equals_brute_force(dev, scene):
+    """bvh_intersect on the packed scene -- CBOX: the coplanar-group test, torus: the BVH walk -- against the minimum of the exact triangle test over every
+    packed triangle, ties to the lower original index (DESIGN.md 2): the same triangle and the same t for every ray.  On the host __fdividef is an exact
+    division, so this checks the packing and the traversal, not the device's approximate pre-filter."""
+    from ppg_b200 import builtin_scenes as B
+    sc = _fixture("cbox") if scene == "cbox" else B.torus_scene(32)
+    rng = np.random.default_rng(21 if scene == "cbox" else 22); n = 20000
+    lo, hi = np.asarray(sc.aabb_min, np.float64), np.asarray(sc.aabb_max, np.float64)
+    o = (lo + (hi - lo) * (0.02 + 0.96 * rng.random((n, 3)))).astype(np.float32)
+    d = rng.normal(size=(n, 3)); d[: n // 10, 1] = 0; d /= np.linalg.norm(d, axis=1, keepdims=True); d = d.astype(np.float32)
+    t = np.zeros((n, 2), np.float32); prim = np.zeros((n, 2), np.uint32)
+    dev.dev_closest_hit.argtypes = [C.c_void_p, C.c_size_t, f32p, f32p, C.c_float, C.c_float, f32p, C.POINTER(C.c_uint32)]
+    with _Packed(dev, sc) as h:
+        assert dev.dev_closest_hit(h, n, o.ctypes.data_as(f32p), d.ctypes.data_as(f32p), 1e-4, np.inf, t.ctypes.data_as(f32p), prim.ctypes.data_as(C.POINTER(C.c_uint32))) == 0
+    hit = prim[:, 1] != 0xFFFFFFFF
+    assert hit.mean() > (0.3 if scene == "cbox" else 0.05)                          # (the box is open towards the camera)
+    assert np.array_equal(prim[:, 0], prim[:, 1]) and np.array_equal(t[:, 0].view(np.uint32), t[:, 1].view(np.uint32))
+
+
+def test_emitter_sampling_and_environment_pdf_on_packed_scenes_match_oracle(dev):
+    """sample_emitter_direct (+ eval_transmittance) and the environment emitter's pdf / radiance of the device source, on the packed scenes of
+    tests/test_gpu_z_envnee.py (env_lit_scene(32); cbox-textured-flat: area + environment light), against the oracle with the same inputs and at that file's
+    tolerances.  Observed on x86-64 with glibc: every direction, value, pdf and distance is bit-equal to the oracle's (the same libm on both sides)."""
+    from ppg_b200 import builtin_scenes as B
+    from common import load_fixture_scene
+    for name, sc in (("env-only", B.env_lit_scene(32)), ("area+env", load_fixture_scene("cbox-textured-flat", 32))):
+        props = dict(sc.integrator, nee="always")
+        o = O.Oracle(O.params_from_xml(props), sc, kind="port")
+        rng = np.random.default_rng(11); n = 100000
+        lo, hi = np.asarray(sc.aabb_min, np.float64), np.asarray(sc.aabb_max, np.float64)
+        ref = (lo + (hi - lo) * (0.1 + 0.8 * rng.random((n, 3)))).astype(np.float32)
+        nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1, keepdims=True); nrm[n // 2:] = 0; nrm = nrm.astype(np.float32)
+        smp = rng.random((n, 2), dtype=np.float32)
+        d = np.zeros((n, 3), np.float32); val = np.zeros((n, 3), np.float32); pdf = np.zeros(n, np.float32); dist = np.zeros(n, np.float32)
+        dev.dev_emitter_sample_direct.argtypes = [C.c_void_p, C.c_size_t, f32p, f32p, f32p, C.c_int, f32p, f32p, f32p, f32p]
+        with _Packed(dev, sc) as h:
+            assert dev.dev_emitter_sample_direct(h, n, ref.ctypes.data_as(f32p), nrm.ctypes.data_as(f32p), smp.ctypes.data_as(f32p), 3,
+                                                 d.ctypes.data_as(f32p), val.ctypes.data_as(f32p), pdf.ctypes.data_as(f32p), dist.ctypes.data_as(f32p)) == 0
+            d0, val0, pdf0, dist0 = o.emitter_sample_direct(ref, nrm, smp, 3)
+            assert np.isfinite(val).all() and np.isfinite(pdf).all() and (pdf0 > 0).mean() > 0.05
+            same = (np.isclose(pdf, pdf0, rtol=1e-4, atol=1e-7) & np.isclose(val, val0, rtol=1e-4, atol=1e-6).all(axis=1) & np.isclose(dist, dist0, rtol=1e-4, atol=1e-5)
+                    & ((np.abs(d - d0).max(axis=1) < 1e-5) | (pdf0 == 0)))
+            assert same.mean() >= 0.998, (name, same.mean())
+            assert abs(float(val.sum()) - float(val0.sum())) <= 2e-3 * float(val0.sum())
+            if name == "env-only":
+                rng = np.random.default_rng(12)
+                q = rng.normal(size=(200000, 3)); q = (q / np.linalg.norm(q, axis=1, keepdims=True)).astype(np.float32)
+                epdf = np.zeros(len(q), np.float32); eval_ = np.zeros((len(q), 3), np.float32)
+                dev.dev_env_pdf.argtypes = [C.c_void_p, C.c_size_t, f32p, f32p, f32p]
+                assert dev.dev_env_pdf(h, len(q), q.ctypes.data_as(f32p), epdf.ctypes.data_as(f32p), eval_.ctypes.data_as(f32p)) == 0
+                epdf0, eval0 = o.env_pdf(q)
+                assert np.isclose(epdf, epdf0, rtol=2e-3, atol=1e-5).mean() >= 0.999
+                assert np.isclose(eval_, eval0, rtol=2e-3, atol=1e-4).all(axis=1).mean() >= 0.999
+                assert abs(float(epdf.sum()) - float(epdf0.sum())) <= 1e-4 * float(epdf0.sum())
