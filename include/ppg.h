@@ -443,6 +443,55 @@ int ppg_op_stree_lookup(int device,
                         const float aabb_min[3], const float aabb_extent[3],
                         const float *points, size_t n, uint32_t *leaf_out, float *size_out);
 
+/* ---- the learning half: the render's own maintenance, commit and Adam kernels on caller-supplied trees ----------------- *
+ * S-tree arrays per node: node_children (2 uint32, child0 == 0: leaf; the split axis cycles x, y, z from the root), and per leaf its
+ * sampling tree (tree_first = root in the sampling pool, tree_count nodes, tree_depth = m_maxDepth, tree_sum / tree_weight = m_atomic),
+ * its building weight and adam = 6 floats {iter, m1, m2, theta, batchAcc, batchGrad} (GP:69-133).  Pools as above. */
+
+/* resetSDTree (GP:1108-1113): stages bit 0 = STree::refine (GP:957-998; split while the building weight exceeds `threshold`),
+ * bit 1 = DTree::reset of every leaf (GP:456-514) with new_max_depth and dtree_threshold.  node_capacity 0: sized as the render sizes it;
+ * a refinement that runs out of it returns PPG_ERR_CUDA.  Outputs: the S-tree after the refine with the inherited per-node fields
+ * (building_weight_out: after the refine, before the reset clears it) and, per leaf, the new building tree (build_first/count/depth into
+ * build_children_out / build_sums_out).  Output arrays hold out_capacity nodes and build_capacity pool nodes; if either is too small the call
+ * returns PPG_ERR_INVALID_ARGUMENT with *n_nodes_out and *n_build_out set to the sizes needed.  Output pointers other than the counts may be NULL. */
+int ppg_op_sdtree_refine_reset(int device, int stages, float threshold, int new_max_depth, float dtree_threshold, size_t node_capacity,
+                               const uint32_t *node_children, size_t n_nodes, const uint32_t *tree_first, const uint32_t *tree_count, const int32_t *tree_depth,
+                               const float *tree_sum, const float *tree_weight, const float *adam, const float *building_weight,
+                               const float *sums, const uint16_t *children, size_t n_pool,
+                               size_t out_capacity, size_t *n_nodes_out, uint32_t *node_children_out, uint32_t *tree_first_out, uint32_t *tree_count_out,
+                               int32_t *tree_depth_out, float *tree_sum_out, float *tree_weight_out, float *adam_out, float *building_weight_out,
+                               uint32_t *build_first_out, uint32_t *build_count_out, int32_t *build_depth_out,
+                               size_t build_capacity, size_t *n_build_out, uint16_t *build_children_out, float *build_sums_out);
+
+/* buildSDTree (GP:1115-1189): DTree::build of every leaf's building tree (build_first/count/depth, building_weight, pool sums/children) and
+ * "sampling = building".  Outputs: the sampling pool (same indices as the building pool), per node m_atomic sum / weight, depth, node count,
+ * mean() > 0, and stats_out = 14 doubles {leaves, leaves with nodes, depth min, depth max, mean min, mean max, weight min, weight max,
+ * nodes min, nodes max, depth sum, mean sum, nodes sum, weight sum} (the "distribution statistics", GP:1121-1186). */
+int ppg_op_sdtree_build(int device, const uint32_t *node_children, size_t n_nodes, const uint32_t *build_first, const uint32_t *build_count,
+                        const int32_t *build_depth, const float *building_weight, const float *sums, const uint16_t *children, size_t n_pool,
+                        float *sampling_sums_out, uint16_t *sampling_children_out, float *tree_sum_out, float *tree_weight_out,
+                        int32_t *tree_depth_out, uint32_t *tree_count_out, uint8_t *mean_positive_out, double *stats_out);
+
+/* Vertex::commit (GP:1730-1768) of n path vertices through the render's commit kernel (record_mode 1: three vertex fields, nearest only;
+ * 2: six).  vertices: 24 floats per vertex, the six float4 the bounce kernel writes {d, woPdf}, {throughput, bits(leaf)},
+ * {radiance prefix, bits(path | absolute << 30 | delta << 31)}, {bsdf value, bsdfPdf}, {o, dTreePdf}, {bits(sampleIndex lo), bits(hi),
+ * bits(S-tree levels | ordinal << 8), 0}; li_final: 4 floats per path.  Building weights and sums are updated in place.  With a loss the
+ * sampling-fraction records are appended to adam_records_out (6 floats: bits(leaf), product, woPdf, bsdfPdf, dTreePdf, weight; up to
+ * adam_capacity), *n_adam_out = records produced. */
+int ppg_op_commit(int device, int record_mode, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
+                  const uint32_t *build_first, float *building_weight_inout, float *sums_inout, const uint16_t *children, size_t n_pool,
+                  const float *vertices, size_t n, const float *li_final, size_t n_li, int spatial_filter, int directional_filter, int loss,
+                  uint64_t seed, float statistical_weight, float *adam_records_out, size_t adam_capacity, size_t *n_adam_out);
+
+/* The sampling-fraction replay (GP:672-697, 85-109) of n_records records (6 floats as ppg_op_commit writes them) into adam states
+ * (state_inout, 6 floats per node).  bucket == 0: the records of node i are records[leaf_offset[i] .. + leaf_count[i]), in that order.
+ * bucket != 0: the records are in any order and are first bucketed by leaf as the render does (histogram, scan, scatter); bucketed_out and
+ * leaf_offset_out then receive the buckets.  theta_out: the per-node theta the sampling kernels read; count_out / cursor_out: the per-leaf
+ * bookkeeping after the replay (zero: ready for the next commit).  loss = PPG_LOSS_KL or PPG_LOSS_VAR.  Output pointers may be NULL. */
+int ppg_op_adam_replay(int device, int loss, int bucket, float *state_inout, size_t n_nodes, const float *records, size_t n_records,
+                       const uint32_t *leaf_offset, const uint32_t *leaf_count, float *theta_out, float *bucketed_out, uint32_t *leaf_offset_out,
+                       uint32_t *count_out, uint32_t *cursor_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -573,6 +573,10 @@ static TreeView tree_view(ppg_integrator *h) {
     return T;
 }
 
+// S-tree node capacity for a refine: a leaf splits only while its weight exceeds the threshold, so the refinement creates at most
+// 4 nodes per threshold worth of building weight
+static double refine_capacity(size_t nodes, double totalWeight, float threshold) { return (double) nodes + 4.0 * totalWeight / std::max(1.0f, threshold) + 1024; }
+
 // resetSDTree, GP:1108-1113
 static int reset_sd_tree(ppg_integrator *h) {
     const double thr = std::sqrt(std::pow(2.0, h->iter) * h->prm.spp_per_pass / 4) * h->prm.s_tree_threshold;
@@ -588,7 +592,7 @@ static int reset_sd_tree(ppg_integrator *h) {
         // capacity: the refinement creates at most 2 nodes per threshold worth of recorded weight.  The total weight of the iteration is at most
         // its number of guiding records (weights <= 1); with several ranks the reduced weights hold about world x this rank's records.
         const double totalW = 1.25 * (double) h->lastRecorded * h->world + 4096;
-        const double est = h->hNodes + 4.0 * totalW / std::max(1.0f, threshold) + 1024;
+        const double est = refine_capacity(h->hNodes, totalW, threshold);
         int rc = ensure_tree_capacity(h, (uint32_t) std::min<double>(est, 4.0e9), h->capPool);
         if (rc) return rc;
         MaintParams M = maint(h);
@@ -1423,4 +1427,239 @@ extern "C" int ppg_op_stree_lookup(int device, const uint32_t *node_children, si
     CK(cudaMemcpy(leaf_out, dl.p, 4 * n, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(size_out, dsz.p, 12 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
+}
+
+// ------------------------------------------------------------------ the learning half: the render's own maintenance, commit and Adam kernels
+namespace {
+static float bits_f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
+static uint32_t f_bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+static int op_sm_count() { int d = 0, n = 0; if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) != cudaSuccess) n = 132; return n; }
+// a zero-filled device array of `cap` elements whose first n are copied from the host (host may be null: zeros)
+template <class T> static cudaError_t dev_array(DevBuf<T> &b, size_t cap, const T *host = nullptr, size_t n = 0) {
+    cudaError_t e = b.alloc(std::max<size_t>(cap, 1)); if (e != cudaSuccess) return e;
+    e = cudaMemset(b.p, 0, std::max<size_t>(cap, 1) * sizeof(T)); if (e != cudaSuccess) return e;
+    return (host && n) ? cudaMemcpy(b.p, host, n * sizeof(T), cudaMemcpyHostToDevice) : cudaSuccess;
+}
+}  // namespace
+
+extern "C" int ppg_op_sdtree_refine_reset(int device, int stages, float threshold, int new_max_depth, float dtree_threshold, size_t node_capacity,
+                                          const uint32_t *node_children, size_t n_nodes, const uint32_t *tree_first, const uint32_t *tree_count, const int32_t *tree_depth,
+                                          const float *tree_sum, const float *tree_weight, const float *adam, const float *building_weight,
+                                          const float *sums, const uint16_t *children, size_t n_pool,
+                                          size_t out_capacity, size_t *n_nodes_out, uint32_t *node_children_out, uint32_t *tree_first_out, uint32_t *tree_count_out,
+                                          int32_t *tree_depth_out, float *tree_sum_out, float *tree_weight_out, float *adam_out, float *building_weight_out,
+                                          uint32_t *build_first_out, uint32_t *build_count_out, int32_t *build_depth_out,
+                                          size_t build_capacity, size_t *n_build_out, uint16_t *build_children_out, float *build_sums_out) {
+  return guarded("ppg_op_sdtree_refine_reset", [&]() -> int {
+    int rc = op_device(device); if (rc) return rc;
+    if (!n_nodes || n_nodes >= 0xFFFFFFFFull || !node_children || !tree_first || !tree_count || !tree_depth || !tree_sum || !tree_weight || !adam || !building_weight ||
+        !sums || !children || !n_pool || !n_nodes_out || !n_build_out)
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: empty or null input");
+    double totalW = 0; for (size_t i = 0; i < n_nodes; ++i) totalW += building_weight[i];
+    const uint32_t cap = node_capacity ? (uint32_t) std::min<size_t>(node_capacity, 0xFFFFFFFFull)
+                                       : std::max<uint32_t>((uint32_t) std::min<double>(refine_capacity(n_nodes, 1.25 * totalW + 4096, threshold), 4.0e9), 1u << 16);
+    if (cap < n_nodes) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: node_capacity below n_nodes");
+    std::vector<float4> la(n_nodes);
+    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(tree_first[i]), 0.f, adam[6 * i + 3], 0.f);
+    std::vector<SampNode> pool = to_pool(sums, children, n_pool);
+    DevBuf<uint2> dS, dBch; DevBuf<float4> dLA, dBs; DevBuf<float> dBW, dSS, dSW, dAd; DevBuf<int> dSD, dBD; DevBuf<uint32_t> dSC, dBC, dBB, dSc; DevBuf<SampNode> dSamp;
+    CK(dev_array(dS, cap, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, cap, la.data(), n_nodes));
+    CK(dev_array(dBW, cap, building_weight, n_nodes)); CK(dev_array(dSS, cap, tree_sum, n_nodes)); CK(dev_array(dSW, cap, tree_weight, n_nodes));
+    CK(dev_array(dSD, cap, tree_depth, n_nodes)); CK(dev_array(dSC, cap, tree_count, n_nodes)); CK(dev_array(dAd, 6 * (size_t) cap, adam, 6 * n_nodes));
+    CK(dev_array(dBC, cap)); CK(dev_array(dBD, cap)); CK(dev_array(dBB, cap)); CK(dev_array(dSamp, n_pool, pool.data(), n_pool));
+    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, 0, 0, 0, 0, 0};
+    CK(dev_array(dSc, 8, sc0, 8));
+    MaintParams M;
+    M.snodes = dS.p; M.leafA = dLA.p; M.bweight = dBW.p; M.sampSum = dSS.p; M.sampWeight = dSW.p; M.sampDepth = dSD.p; M.sampCount = dSC.p; M.adam = dAd.p;
+    M.buildCount = dBC.p; M.buildDepth = dBD.p; M.nNodes = dSc.p; M.capNodes = cap; M.samp = dSamp.p; M.bchildren = nullptr; M.bsums = nullptr;
+    if (stages & 1) stree_refine_kernel<<<1, 1024>>>(M, threshold, dSc.p + 5);        // launch shapes of reset_sd_tree
+    CK(cudaGetLastError());
+    uint32_t hs[8]; CK(cudaMemcpy(hs, dSc.p, 32, cudaMemcpyDeviceToHost));
+    if (hs[5]) return fail(PPG_ERR_CUDA, "S-tree refinement ran out of node capacity");
+    const size_t N = hs[0];
+    std::vector<float> bwRefined(N); CK(cudaMemcpy(bwRefined.data(), dBW.p, 4 * N, cudaMemcpyDeviceToHost));      // leaf_after_reset_kernel zeroes it
+    size_t total = 0;
+    if (stages & 2) {
+        const int blocks = op_sm_count() * 4;
+        dtree_reset_kernel<false><<<blocks, 128>>>(M, nullptr, new_max_depth, dtree_threshold);
+        exclusive_scan_kernel<<<1, 1024>>>(dBC.p, dBB.p, dSc.p, dSc.p + 1);
+        CK(cudaGetLastError());
+        CK(cudaMemcpy(hs, dSc.p, 32, cudaMemcpyDeviceToHost)); total = hs[1];
+        CK(dev_array(dBch, total)); CK(dev_array(dBs, total));
+        M.bchildren = dBch.p; M.bsums = dBs.p;
+        dtree_reset_kernel<true><<<blocks, 128>>>(M, dBB.p, new_max_depth, dtree_threshold);
+        leaf_after_reset_kernel<<<blocks, 256>>>(M, dBB.p);
+        CK(cudaGetLastError());
+    }
+    *n_nodes_out = N; *n_build_out = total;
+    if (N > out_capacity || total > build_capacity)
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: output arrays too small (*n_nodes_out and *n_build_out hold the sizes needed)");
+    std::vector<float4> laOut(N); CK(cudaMemcpy(laOut.data(), dLA.p, 16 * N, cudaMemcpyDeviceToHost));
+    if (tree_first_out) for (size_t i = 0; i < N; ++i) tree_first_out[i] = f_bits(laOut[i].x);
+    if (node_children_out) CK(cudaMemcpy(node_children_out, dS.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (tree_count_out) CK(cudaMemcpy(tree_count_out, dSC.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, dSD.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, dSS.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, dSW.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (adam_out) CK(cudaMemcpy(adam_out, dAd.p, 24 * N, cudaMemcpyDeviceToHost));
+    if (building_weight_out) memcpy(building_weight_out, bwRefined.data(), 4 * N);
+    if (build_first_out) CK(cudaMemcpy(build_first_out, dBB.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_count_out) CK(cudaMemcpy(build_count_out, dBC.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_depth_out) CK(cudaMemcpy(build_depth_out, dBD.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_children_out && total) CK(cudaMemcpy(build_children_out, dBch.p, 8 * total, cudaMemcpyDeviceToHost));     // uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
+    if (build_sums_out && total) CK(cudaMemcpy(build_sums_out, dBs.p, 16 * total, cudaMemcpyDeviceToHost));
+    return PPG_OK;
+  });
+}
+
+extern "C" int ppg_op_sdtree_build(int device, const uint32_t *node_children, size_t n_nodes, const uint32_t *build_first, const uint32_t *build_count,
+                                   const int32_t *build_depth, const float *building_weight, const float *sums, const uint16_t *children, size_t n_pool,
+                                   float *sampling_sums_out, uint16_t *sampling_children_out, float *tree_sum_out, float *tree_weight_out,
+                                   int32_t *tree_depth_out, uint32_t *tree_count_out, uint8_t *mean_positive_out, double *stats_out) {
+  return guarded("ppg_op_sdtree_build", [&]() -> int {
+    int rc = op_device(device); if (rc) return rc;
+    if (!n_nodes || n_nodes >= 0xFFFFFFFFull || !node_children || !build_first || !build_count || !build_depth || !building_weight || !sums || !children || !n_pool)
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_build: empty or null input");
+    std::vector<float4> la(n_nodes);
+    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(build_first[i]), bits_f(build_first[i]), 0.f, 0.f);
+    DevBuf<uint2> dS, dBch; DevBuf<float4> dLA, dBs; DevBuf<float> dBW, dSS, dSW; DevBuf<int> dSD, dBD; DevBuf<uint32_t> dSC, dBC, dBB, dSc; DevBuf<SampNode> dSamp;
+    DevBuf<TreeStats> dTS;
+    CK(dev_array(dS, n_nodes, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, n_nodes, la.data(), n_nodes));
+    CK(dev_array(dBW, n_nodes, building_weight, n_nodes)); CK(dev_array(dSS, n_nodes)); CK(dev_array(dSW, n_nodes)); CK(dev_array(dSD, n_nodes)); CK(dev_array(dSC, n_nodes));
+    CK(dev_array(dBC, n_nodes, build_count, n_nodes)); CK(dev_array(dBD, n_nodes, build_depth, n_nodes)); CK(dev_array(dBB, n_nodes, build_first, n_nodes));
+    CK(dev_array(dBch, n_pool, reinterpret_cast<const uint2 *>(children), n_pool)); CK(dev_array(dBs, n_pool, reinterpret_cast<const float4 *>(sums), n_pool));
+    CK(dev_array(dSamp, n_pool)); CK(dev_array(dTS, 1));
+    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, 0, 0, 0, 0, 0};
+    CK(dev_array(dSc, 8, sc0, 8));
+    MaintParams M;
+    M.snodes = dS.p; M.leafA = dLA.p; M.bweight = dBW.p; M.sampSum = dSS.p; M.sampWeight = dSW.p; M.sampDepth = dSD.p; M.sampCount = dSC.p; M.adam = nullptr;
+    M.buildCount = dBC.p; M.buildDepth = dBD.p; M.nNodes = dSc.p; M.capNodes = (uint32_t) n_nodes; M.samp = dSamp.p; M.bchildren = dBch.p; M.bsums = dBs.p;
+    dtree_build_kernel<<<op_sm_count() * 4, 128>>>(M, dBB.p);        // launch shapes of build_sd_tree
+    tree_stats_kernel<<<1, 1024>>>(M, dTS.p);
+    CK(cudaGetLastError());
+    std::vector<SampNode> pool(n_pool); CK(cudaMemcpy(pool.data(), dSamp.p, sizeof(SampNode) * n_pool, cudaMemcpyDeviceToHost));
+    for (size_t k = 0; k < n_pool; ++k) {
+        if (sampling_sums_out) memcpy(sampling_sums_out + 4 * k, &pool[k].sums, 16);
+        if (sampling_children_out) memcpy(sampling_children_out + 4 * k, &pool[k].children, 8);
+    }
+    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, dSS.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, dSW.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, dSD.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (tree_count_out) CK(cudaMemcpy(tree_count_out, dSC.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (mean_positive_out) {
+        std::vector<float4> laOut(n_nodes); CK(cudaMemcpy(laOut.data(), dLA.p, 16 * n_nodes, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n_nodes; ++i) mean_positive_out[i] = f_bits(laOut[i].w) != 0u;
+    }
+    if (stats_out) {
+        TreeStats t; CK(cudaMemcpy(&t, dTS.p, sizeof(t), cudaMemcpyDeviceToHost));
+        const double v[14] = {(double) t.leaves, (double) t.leavesWithNodes, (double) t.depthMin, (double) t.depthMax, t.meanMin, t.meanMax, t.weightMin, t.weightMax,
+                              (double) t.nodesMin, (double) t.nodesMax, t.depthSum, t.meanSum, t.nodesSum, t.weightSum};
+        memcpy(stats_out, v, sizeof(v));
+    }
+    return PPG_OK;
+  });
+}
+
+extern "C" int ppg_op_commit(int device, int record_mode, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
+                             const uint32_t *build_first, float *building_weight_inout, float *sums_inout, const uint16_t *children, size_t n_pool,
+                             const float *vertices, size_t n, const float *li_final, size_t n_li, int spatial_filter, int directional_filter, int loss,
+                             uint64_t seed, float statistical_weight, float *adam_records_out, size_t adam_capacity, size_t *n_adam_out) {
+  return guarded("ppg_op_commit", [&]() -> int {
+    int rc = op_device(device); if (rc) return rc;
+    if (record_mode != 1 && record_mode != 2) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_commit: record_mode is 1 (nearest, 3 vertex fields) or 2 (6 fields)");
+    if (!n_nodes || !node_children || !aabb_min || !aabb_extent || !build_first || !building_weight_inout || !sums_inout || !children || !n_pool ||
+        (n && (!vertices || !li_final)) || n >= 0x40000000ull || !n_adam_out)
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_commit: empty or null input");
+    std::vector<float4> la(n_nodes);
+    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(build_first[i]), bits_f(build_first[i]), 0.f, 0.f);
+    // the bounce kernel's slab layout: field f of vertex i at f * n + i
+    std::vector<float4> slab(6 * std::max<size_t>(n, 1));
+    for (size_t i = 0; i < n; ++i)
+        for (int f = 0; f < 6; ++f) memcpy(&slab[(size_t) f * n + i], vertices + 24 * i + 4 * f, 16);
+    const uint32_t live = (uint32_t) n, cap = (uint32_t) std::min<size_t>(adam_capacity, 0xFFFFFFFFull);
+    DevBuf<uint2> dS, dBch; DevBuf<uint32_t> dTab, dLive, dTot; DevBuf<float4> dLA, dBs, dSlab, dLi, dRA; DevBuf<float> dBW; DevBuf<float2> dRB; DevBuf<unsigned long long> dDrop;
+    CK(dev_array(dS, n_nodes, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, n_nodes, la.data(), n_nodes));
+    CK(dev_array(dBW, n_nodes, building_weight_inout, n_nodes));
+    CK(dev_array(dBch, n_pool, reinterpret_cast<const uint2 *>(children), n_pool)); CK(dev_array(dBs, n_pool, reinterpret_cast<const float4 *>(sums_inout), n_pool));
+    CK(dev_array(dSlab, slab.size(), slab.data(), slab.size())); CK(dev_array(dLi, n_li, reinterpret_cast<const float4 *>(li_final), n_li));
+    CK(dev_array(dLive, 1, &live, 1)); CK(dev_array(dTot, 1)); CK(dev_array(dDrop, 1)); CK(dev_array(dRA, cap)); CK(dev_array(dRB, cap));
+    CK(dev_array(dTab, (size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
+    stree_table_kernel<<<296, 256>>>(dS.p, dTab.p);        // as after every refine (reset_sd_tree)
+    CommitParams C; memset(&C, 0, sizeof(C));
+    C.tree.snodes = dS.p; C.tree.stable = dTab.p; C.tree.leafA = dLA.p; C.tree.samp = nullptr; C.tree.bchildren = dBch.p; C.tree.bsums = dBs.p; C.tree.bweight = dBW.p;
+    C.tree.aabbMin = make_float3(aabb_min[0], aabb_min[1], aabb_min[2]); C.tree.extent = make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]);
+    VertexSlab S; float4 *b = dSlab.p;
+    S.v0 = b; S.v1 = b + n; S.v2 = b + 2 * n; S.v3 = b + 3 * n; S.v4 = b + 4 * n; S.v5 = b + 5 * n;
+    C.slab0 = S; C.slabStride = n; C.liveCounts = dLive.p; C.liFinal = dLi.p;
+    C.spatialFilter = spatial_filter; C.directionalFilter = directional_filter; C.lossMode = loss; C.statisticalWeight = statistical_weight;
+    C.nee0 = S; C.nSlabs = 1; C.seed = seed; C.snodes = dS.p;
+    C.adamRecA = dRA.p; C.adamRecB = dRB.p; C.adamTotal = dTot.p; C.adamCap = cap; C.dropped = dDrop.p;
+    if (n) {
+        int occ = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, commit_kernel<1>, PPG_BLOCK, 0));       // grid of render_batch
+        const dim3 g(std::min<int>(op_sm_count() * std::max(occ, 1), (int) ((n + PPG_BLOCK - 1) / PPG_BLOCK)), 1);
+        if (record_mode == 1) commit_kernel<1><<<g, PPG_BLOCK>>>(C); else commit_kernel<2><<<g, PPG_BLOCK>>>(C);
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(sums_inout, dBs.p, 16 * n_pool, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(building_weight_inout, dBW.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    uint32_t tot = 0; CK(cudaMemcpy(&tot, dTot.p, 4, cudaMemcpyDeviceToHost));
+    *n_adam_out = tot;
+    const size_t kept = std::min<size_t>(tot, cap);
+    if (adam_records_out && kept) {
+        std::vector<float4> ra(kept); std::vector<float2> rb(kept);
+        CK(cudaMemcpy(ra.data(), dRA.p, 16 * kept, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), dRB.p, 8 * kept, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < kept; ++i) { memcpy(adam_records_out + 6 * i, &ra[i], 16); memcpy(adam_records_out + 6 * i + 4, &rb[i], 8); }
+    }
+    return PPG_OK;
+  });
+}
+
+extern "C" int ppg_op_adam_replay(int device, int loss, int bucket, float *state_inout, size_t n_nodes, const float *records, size_t n_records,
+                                  const uint32_t *leaf_offset, const uint32_t *leaf_count, float *theta_out, float *bucketed_out, uint32_t *leaf_offset_out,
+                                  uint32_t *count_out, uint32_t *cursor_out) {
+  return guarded("ppg_op_adam_replay", [&]() -> int {
+    int rc = op_device(device); if (rc) return rc;
+    if (loss != PPG_LOSS_KL && loss != PPG_LOSS_VAR) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: loss is kl or var");
+    if (!state_inout || !n_nodes || n_nodes >= 0xFFFFFFFFull || n_records >= 0xFFFFFFFFull || (n_records && !records) || (!bucket && (!leaf_offset || !leaf_count)))
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: empty or null input");
+    std::vector<float4> ra(std::max<size_t>(n_records, 1)); std::vector<float2> rb(std::max<size_t>(n_records, 1));
+    for (size_t i = 0; i < n_records; ++i) { memcpy(&ra[i], records + 6 * i, 16); memcpy(&rb[i], records + 6 * i + 4, 8); }
+    std::vector<float4> la(n_nodes);
+    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(0.f, 0.f, state_inout[6 * i + 3], 0.f);
+    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, (uint32_t) n_records, 0, 0, 0, 0};
+    DevBuf<float4> dLA, dRA, dSA; DevBuf<float2> dRB, dSB; DevBuf<float> dAd; DevBuf<uint32_t> dCount, dCursor, dOff, dSc;
+    CK(dev_array(dLA, n_nodes, la.data(), n_nodes)); CK(dev_array(dAd, 6 * n_nodes, state_inout, 6 * n_nodes)); CK(dev_array(dSc, 8, sc0, 8));
+    CK(dev_array(dRA, n_records, ra.data(), n_records)); CK(dev_array(dRB, n_records, rb.data(), n_records));
+    MaintParams M; memset(&M, 0, sizeof(M));
+    M.leafA = dLA.p; M.adam = dAd.p; M.nNodes = dSc.p; M.capNodes = (uint32_t) n_nodes;
+    const int sms = op_sm_count();
+    if (bucket) {       // render_batch: histogram -> scan -> scatter into per-leaf buckets
+        CK(dev_array(dCount, n_nodes)); CK(dev_array(dCursor, n_nodes)); CK(dev_array(dOff, n_nodes)); CK(dev_array(dSA, n_records)); CK(dev_array(dSB, n_records));
+        adam_hist_kernel<<<sms * 4, 256>>>(dRA.p, dSc.p + 3, (uint32_t) n_records, dCount.p);
+        exclusive_scan_kernel<<<1, 1024>>>(dCount.p, dOff.p, dSc.p, dSc.p + 4);
+        adam_scatter_kernel<<<sms * 4, 256>>>(dRA.p, dRB.p, dSc.p + 3, (uint32_t) n_records, dOff.p, dCursor.p, dSA.p, dSB.p);
+        CK(cudaGetLastError());
+        if (bucketed_out && n_records) {
+            CK(cudaMemcpy(ra.data(), dSA.p, 16 * n_records, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), dSB.p, 8 * n_records, cudaMemcpyDeviceToHost));
+            for (size_t i = 0; i < n_records; ++i) { memcpy(bucketed_out + 6 * i, &ra[i], 16); memcpy(bucketed_out + 6 * i + 4, &rb[i], 8); }
+        }
+        if (leaf_offset_out) CK(cudaMemcpy(leaf_offset_out, dOff.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    } else {            // records already grouped; the cursors hold the counts, as after adam_scatter_kernel
+        for (size_t i = 0; i < n_nodes; ++i)
+            if ((size_t) leaf_offset[i] + leaf_count[i] > n_records) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: a leaf's records run past n_records");
+        CK(dev_array(dCount, n_nodes, leaf_count, n_nodes)); CK(dev_array(dCursor, n_nodes, leaf_count, n_nodes)); CK(dev_array(dOff, n_nodes, leaf_offset, n_nodes));
+        if (leaf_offset_out) memcpy(leaf_offset_out, leaf_offset, 4 * n_nodes);
+    }
+    adam_seq_kernel<<<sms * 16, 128>>>(M, bucket ? dSA.p : dRA.p, bucket ? dSB.p : dRB.p, dOff.p, dCount.p, dCursor.p, loss == PPG_LOSS_KL ? 1.0f : 2.0f);
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(state_inout, dAd.p, 24 * n_nodes, cudaMemcpyDeviceToHost));
+    if (theta_out) {
+        CK(cudaMemcpy(la.data(), dLA.p, 16 * n_nodes, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n_nodes; ++i) theta_out[i] = la[i].z;
+    }
+    if (count_out) CK(cudaMemcpy(count_out, dCount.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (cursor_out) CK(cudaMemcpy(cursor_out, dCursor.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    return PPG_OK;
+  });
 }

@@ -288,9 +288,12 @@ __global__ void __launch_bounds__(1024) stree_refine_kernel(const __grid_constan
             if (threadIdx.x == 0) { sBase = min(base + 2 * total, M.capNodes & ~1u); if (total) sAny = 1; }
             __syncthreads();
         }
+        // The loop condition is taken into registers BEFORE the barrier: thread 0 resets sAny and sBase at the top of the next
+        // round, and a warp that read them after that barrier could leave the loop while the others carry on.
+        const bool more = sAny && end < sBase;
         if (threadIdx.x == 0) { sBegin = end; sEnd = sBase; }
         __syncthreads();
-        if (!sAny || sBegin >= sEnd) break;
+        if (!more) break;
     }
     if (threadIdx.x == 0) *M.nNodes = sEnd;
 }

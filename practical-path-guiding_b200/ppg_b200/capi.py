@@ -224,6 +224,13 @@ def load_library(path: str | None = None):
     lib.ppg_op_bvh_build.argtypes = [f32p, u32p, C.c_size_t, C.c_int, f32p, C.c_size_t, u32p, C.POINTER(C.c_size_t), C.POINTER(C.c_int), C.POINTER(C.c_double)]
     lib.ppg_op_emitter_sample_direct.argtypes = [H, C.c_size_t, f32p, f32p, f32p, C.c_int, f32p, f32p, f32p, f32p]
     lib.ppg_op_env_pdf.argtypes = [H, C.c_size_t, f32p, f32p, f32p]
+    i32p = C.POINTER(C.c_int32); u8p = C.POINTER(C.c_uint8); szp = C.POINTER(C.c_size_t); sz = C.c_size_t
+    lib.ppg_op_sdtree_refine_reset.argtypes = [C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, sz, u32p, sz, u32p, u32p, i32p, f32p, f32p, f32p, f32p, f32p, u16p, sz,
+                                               sz, szp, u32p, u32p, u32p, i32p, f32p, f32p, f32p, f32p, u32p, u32p, i32p, sz, szp, u16p, f32p]
+    lib.ppg_op_sdtree_build.argtypes = [C.c_int, u32p, sz, u32p, u32p, i32p, f32p, f32p, u16p, sz, f32p, u16p, f32p, f32p, i32p, u32p, u8p, C.POINTER(C.c_double)]
+    lib.ppg_op_commit.argtypes = [C.c_int, C.c_int, u32p, sz, f32p, f32p, u32p, f32p, f32p, u16p, sz, f32p, sz, f32p, sz, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_float,
+                                  f32p, sz, szp]
+    lib.ppg_op_adam_replay.argtypes = [C.c_int, C.c_int, C.c_int, f32p, sz, f32p, sz, u32p, u32p, f32p, f32p, u32p, u32p, u32p]
     if path is None:
         _lib = lib
     return lib
@@ -234,4 +241,5 @@ EXPORTED_SYMBOLS = [
     "ppg_destroy", "ppg_scene_file_load", "ppg_scene_file_free", "ppg_set_scene", "ppg_set_shard", "ppg_set_allreduce", "ppg_nccl_unique_id", "ppg_nccl_init", "ppg_set_clock", "ppg_set_film_callback", "ppg_render", "ppg_render_device", "ppg_cancel",
     "ppg_copy_from_device", "ppg_dump_sdtree", "ppg_set_destination", "ppg_get_moment_images", "ppg_last_error", "ppg_op_dtree_pdf", "ppg_op_dtree_sample",
     "ppg_op_dtree_record", "ppg_op_stree_lookup", "ppg_op_emitter_sample_direct", "ppg_op_env_pdf", "ppg_op_bvh_build",
+    "ppg_op_sdtree_refine_reset", "ppg_op_sdtree_build", "ppg_op_commit", "ppg_op_adam_replay",
 ]

@@ -230,6 +230,96 @@ def op_dtree_record(sums, children, tree_first, tree_weight, rec_tree, rec_dir, 
     return sums, tw
 
 
+def _c(a, dt):
+    return np.ascontiguousarray(a, dt)
+
+
+TREE_STATS = ("leaves", "leaves_with_nodes", "depth_min", "depth_max", "mean_min", "mean_max", "weight_min", "weight_max",
+              "nodes_min", "nodes_max", "depth_sum", "mean_sum", "nodes_sum", "weight_sum")
+
+
+def op_sdtree_refine_reset(tree, building_weight, threshold, refine=True, reset=True, new_max_depth=20, dtree_threshold=0.01, node_capacity=0, device=0):
+    """STree::refine and/or DTree::reset of every leaf through the render's kernels (ppg_op_sdtree_refine_reset).  `tree`: the sampling half of an
+    S-tree as a dict of flat arrays (s_children, tree_first/count/depth/sum/weight, adam, sums, children); `building_weight` per node.
+    Returns a dict of the new S-tree: s_children, tree_first/count/depth/sum/weight, adam, building_weight (after the refine) and the new
+    building trees: build_first/count/depth, build_children, build_sums."""
+    lib = capi.load_library()
+    sch = _c(tree["s_children"], np.uint32); n = len(sch)
+    ins = [_c(tree["tree_first"], np.uint32), _c(tree["tree_count"], np.uint32), _c(tree["tree_depth"], np.int32), _c(tree["tree_sum"], np.float32),
+           _c(tree["tree_weight"], np.float32), _c(tree["adam"], np.float32), _c(building_weight, np.float32)]
+    sums = _c(tree["sums"], np.float32); ch = _c(tree["children"], np.uint16)
+    cap, bcap = max(2 * n, 1024), max(4 * len(sums), 1024)
+    nn, nb = C.c_size_t(), C.c_size_t()
+    for _ in range(2):
+        o = dict(s_children=np.zeros((cap, 2), np.uint32), tree_first=np.zeros(cap, np.uint32), tree_count=np.zeros(cap, np.uint32), tree_depth=np.zeros(cap, np.int32),
+                 tree_sum=np.zeros(cap, np.float32), tree_weight=np.zeros(cap, np.float32), adam=np.zeros((cap, 6), np.float32), building_weight=np.zeros(cap, np.float32),
+                 build_first=np.zeros(cap, np.uint32), build_count=np.zeros(cap, np.uint32), build_depth=np.zeros(cap, np.int32),
+                 build_children=np.zeros((bcap, 4), np.uint16), build_sums=np.zeros((bcap, 4), np.float32))
+        T = (C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_uint32, C.c_uint32, C.c_int32)
+        keys = ("s_children", "tree_first", "tree_count", "tree_depth", "tree_sum", "tree_weight", "adam", "building_weight", "build_first", "build_count", "build_depth")
+        rc = lib.ppg_op_sdtree_refine_reset(device, (1 if refine else 0) | (2 if reset else 0), threshold, new_max_depth, dtree_threshold, node_capacity,
+                                            _p(sch, C.c_uint32), n, *[_p(a, t) for a, t in zip(ins, (C.c_uint32, C.c_uint32, C.c_int32) + (C.c_float,) * 4)],
+                                            _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), cap, C.byref(nn), *[_p(o[k], t) for k, t in zip(keys, T)],
+                                            bcap, C.byref(nb), _p(o["build_children"], C.c_uint16), _p(o["build_sums"], C.c_float))
+        if rc == -1 and (nn.value > cap or nb.value > bcap):
+            cap, bcap = max(cap, nn.value), max(bcap, nb.value)
+            continue
+        _check(lib, rc)
+        break
+    o = {k: (v[:nb.value] if k in ("build_children", "build_sums") else v[:nn.value]) for k, v in o.items()}
+    return o
+
+
+def op_sdtree_build(s_children, build_first, build_count, build_depth, building_weight, sums, children, device=0):
+    """DTree::build of every leaf + "sampling = building" + the distribution statistics through the render's kernels (ppg_op_sdtree_build).
+    Returns (sampling sums, sampling children, dict of per-node tree_sum / tree_weight / tree_depth / tree_count / mean_positive, stats dict)."""
+    lib = capi.load_library()
+    sch = _c(s_children, np.uint32); n = len(sch)
+    bf, bc, bd, bw = _c(build_first, np.uint32), _c(build_count, np.uint32), _c(build_depth, np.int32), _c(building_weight, np.float32)
+    sums = _c(sums, np.float32); ch = _c(children, np.uint16)
+    ss, sc = np.zeros_like(sums), np.zeros_like(ch)
+    per = dict(tree_sum=np.zeros(n, np.float32), tree_weight=np.zeros(n, np.float32), tree_depth=np.zeros(n, np.int32), tree_count=np.zeros(n, np.uint32),
+               mean_positive=np.zeros(n, np.uint8))
+    st = np.zeros(14, np.float64)
+    _check(lib, lib.ppg_op_sdtree_build(device, _p(sch, C.c_uint32), n, _p(bf, C.c_uint32), _p(bc, C.c_uint32), _p(bd, C.c_int32), _p(bw, C.c_float),
+                                        _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), _p(ss, C.c_float), _p(sc, C.c_uint16),
+                                        _p(per["tree_sum"], C.c_float), _p(per["tree_weight"], C.c_float), _p(per["tree_depth"], C.c_int32),
+                                        _p(per["tree_count"], C.c_uint32), _p(per["mean_positive"], C.c_uint8), _p(st, C.c_double)))
+    return ss, sc, per, dict(zip(TREE_STATS, st.tolist()))
+
+
+def op_commit(s_children, aabb_min, aabb_extent, build_first, building_weight, sums, children, vertices, li_final, record_mode=2, spatial_filter=0,
+              directional_filter=0, loss=0, seed=0, statistical_weight=1.0, adam_capacity=None, device=0):
+    """Vertex::commit of the vertices (n, 6, 4) float32 -- the six float4 the bounce kernel writes -- through the render's commit kernel
+    (ppg_op_commit).  Returns (building sums, building weights, sampling-fraction records (m, 6) float32 with the leaf's bits in column 0)."""
+    lib = capi.load_library()
+    sch = _c(s_children, np.uint32); mn = _c(aabb_min, np.float32); ex = _c(aabb_extent, np.float32); bf = _c(build_first, np.uint32)
+    bw = np.array(building_weight, np.float32, copy=True, order="C"); sums = np.array(sums, np.float32, copy=True, order="C"); ch = _c(children, np.uint16)
+    v = _c(vertices, np.float32).reshape(-1, 24); li = _c(li_final, np.float32).reshape(-1, 4)
+    cap = len(v) * 64 if adam_capacity is None else adam_capacity
+    rec = np.zeros((max(cap, 1), 6), np.float32); na = C.c_size_t()
+    _check(lib, lib.ppg_op_commit(device, record_mode, _p(sch, C.c_uint32), len(sch), _p(mn, C.c_float), _p(ex, C.c_float), _p(bf, C.c_uint32), _p(bw, C.c_float),
+                                  _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), _p(v, C.c_float), len(v), _p(li, C.c_float), len(li), spatial_filter,
+                                  directional_filter, loss, seed, statistical_weight, _p(rec, C.c_float), cap, C.byref(na)))
+    return sums, bw, rec[:min(na.value, cap)]
+
+
+def op_adam_replay(state, records, loss, leaf_offset=None, leaf_count=None, bucket=False, device=0):
+    """The sampling-fraction replay (adam_seq_kernel) of records (m, 6) float32 into the per-node states (n, 6) (ppg_op_adam_replay).  Without
+    `bucket` the records of node i are records[leaf_offset[i]:leaf_offset[i] + leaf_count[i]]; with it they are bucketed by leaf first, as the render
+    does.  Returns a dict: state, theta, count, cursor, and with `bucket` the buckets (records) and their offsets (leaf_offset)."""
+    lib = capi.load_library()
+    st = np.array(state, np.float32, copy=True, order="C").reshape(-1, 6); n = len(st)
+    rec = _c(records, np.float32).reshape(-1, 6)
+    off = None if leaf_offset is None else _c(leaf_offset, np.uint32); cnt = None if leaf_count is None else _c(leaf_count, np.uint32)
+    o = dict(theta=np.zeros(n, np.float32), records=np.zeros_like(rec), leaf_offset=np.zeros(n, np.uint32), count=np.zeros(n, np.uint32), cursor=np.zeros(n, np.uint32))
+    _check(lib, lib.ppg_op_adam_replay(device, loss, 1 if bucket else 0, _p(st, C.c_float), n, _p(rec, C.c_float), len(rec),
+                                       None if off is None else _p(off, C.c_uint32), None if cnt is None else _p(cnt, C.c_uint32), _p(o["theta"], C.c_float),
+                                       _p(o["records"], C.c_float), _p(o["leaf_offset"], C.c_uint32), _p(o["count"], C.c_uint32), _p(o["cursor"], C.c_uint32)))
+    o["state"] = st
+    return o
+
+
 def op_bvh_build(positions, indices, threads=0):
     """The BVH ppg_set_scene builds, on the host (no device): (nodes (N,8) float32, order (T,) uint32, max depth, milliseconds)."""
     lib = capi.load_library()

@@ -3,6 +3,20 @@ import os
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CUDA_INC = next((p for p in (os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include"), "/usr/local/cuda/include") if os.path.exists(os.path.join(p, "cuda_runtime.h"))), None)
+
+
+def compile_device_on_host(so):
+    """tests/hostdev/device_on_host.cpp -- the product's device source compiled for the host with g++ (CUDA's headers supply the vector types) -- as the
+    shared library `so`; returns the ctypes handle."""
+    import ctypes
+    import subprocess
+    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I" + CUDA_INC, "-D__device__=", "-D__host__=", "-D__global__=", "-D__shared__=",
+           "-D__forceinline__=inline", "-D__noinline__=", "-D__launch_bounds__(...)=", "-Wno-unused-function", os.path.join(ROOT, "tests", "hostdev", "device_on_host.cpp"),
+           os.path.join(ROOT, "practical-path-guiding_b200", "csrc", "ppg_scene.cpp"), "-o", str(so)]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-3000:]
+    return ctypes.CDLL(str(so))
 
 
 def assert_render_parity(img, ref, st, ost, sc=None, props=None, pixels=0.90, mean=0.01, counts=2e-4, leaves=1):

@@ -147,6 +147,14 @@ int dev_dtree(const float *sums, const uint16_t *children, size_t n_nodes, const
     }
     return 0;
 }
+// the stochastic spatial filter's jitter of commit_kernel: the three uniforms of the vertex stream seed_vertex_rng(seed, sampleIndex, ordinal)
+int dev_vertex_jitter(uint64_t seed, size_t n, const uint64_t *sample_index, const uint32_t *ordinal, float *out) {
+    for (size_t i = 0; i < n; ++i) {
+        Pcg32 r; seed_vertex_rng(r, seed, sample_index[i], ordinal[i]);
+        out[3 * i] = r.next1D(); out[3 * i + 1] = r.next1D(); out[3 * i + 2] = r.next1D();
+    }
+    return 0;
+}
 // ---- packed scenes: nearest hit, light sampling, environment emitter
 // bvh_intersect (coplanar groups or BVH walk, whichever the packing chose), and the brute-force minimum of tri_intersect over every packed accel row
 // (ties to the lower original triangle index).  t_out / prim_out: 2 per ray {bvh_intersect, brute force}; prim 0xFFFFFFFF = miss.

@@ -14,22 +14,15 @@ import numpy as np
 import pytest
 
 import oracle_lib as O
-from common import ROOT
+from common import CUDA_INC, ROOT, compile_device_on_host
 
-CUDA_INC = next((p for p in (os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include"), "/usr/local/cuda/include") if os.path.exists(os.path.join(p, "cuda_runtime.h"))), None)
 pytestmark = pytest.mark.skipif(CUDA_INC is None or shutil.which("g++") is None, reason="needs g++ and the CUDA headers")
 f32p = C.POINTER(C.c_float)
 
 
 @pytest.fixture(scope="module")
 def dev(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("hostdev") / "libdevice_on_host.so")
-    cmd = ["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I" + CUDA_INC, "-D__device__=", "-D__host__=", "-D__global__=", "-D__shared__=",
-           "-D__forceinline__=inline", "-D__noinline__=", "-D__launch_bounds__(...)=", "-Wno-unused-function", os.path.join(ROOT, "tests", "hostdev", "device_on_host.cpp"),
-           os.path.join(ROOT, "practical-path-guiding_b200", "csrc", "ppg_scene.cpp"), "-o", so]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
+    lib = compile_device_on_host(tmp_path_factory.mktemp("hostdev") / "libdevice_on_host.so")
     lib.dev_scene_open.restype = C.c_void_p; lib.dev_scene_open.argtypes = [C.c_void_p]
     lib.dev_scene_close.restype = None; lib.dev_scene_close.argtypes = [C.c_void_p]
     return lib
@@ -439,3 +432,43 @@ def test_emitter_sampling_and_environment_pdf_on_packed_scenes_match_oracle(dev)
                 assert np.isclose(epdf, epdf0, rtol=2e-3, atol=1e-5).mean() >= 0.999
                 assert np.isclose(eval_, eval0, rtol=2e-3, atol=1e-4).all(axis=1).mean() >= 0.999
                 assert abs(float(epdf.sum()) - float(epdf0.sum())) <= 1e-4 * float(epdf0.sum())
+
+
+def _pcg_vertex_jitter(seed, sample_index, ordinal):
+    """PCG32 (O'Neill's pcg32_random_r with the splitmix64 keying of seed_vertex_rng), restated on Python integers: three next1D()."""
+    M = (1 << 64) - 1
+
+    def splitmix(x):
+        x = (x + 0x9E3779B97F4A7C15) & M
+        x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & M
+        x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & M
+        return x ^ (x >> 31)
+
+    key = (sample_index * 64 + ordinal) & M
+    state, inc = 0, ((key << 1) | 1) & M
+
+    def nxt():
+        nonlocal state
+        old = state
+        state = (old * 6364136223846793005 + inc) & M
+        xs = (((old >> 18) ^ old) >> 27) & 0xFFFFFFFF
+        rot = old >> 59
+        return ((xs >> rot) | (xs << ((32 - rot) & 31))) & 0xFFFFFFFF
+
+    nxt(); state = (state + splitmix(((seed + 0x5851F42D4C957F2D) & M) ^ splitmix(key))) & M; nxt()
+    return [np.float32(nxt() >> 8) * np.float32(1.0 / 16777216.0) for _ in range(3)]
+
+
+def test_vertex_jitter_source_is_pcg32_of_the_vertex_stream(dev):
+    """dev_vertex_jitter -- the uniforms commit_kernel's stochastic spatial filter draws from seed_vertex_rng(seed, sampleIndex, ordinal), which the GPU
+    commit tests hand to the oracle -- equals PCG32 restated on Python integers, bit for bit, including 64-bit sample indices and ordinals up to 2^24."""
+    rng = np.random.default_rng(21); n = 300
+    si = rng.integers(0, 1 << 63, n, dtype=np.uint64); si[:4] = [0, 1, (1 << 32) - 1, (1 << 64) - 1]
+    od = rng.integers(0, 1 << 24, n, dtype=np.uint32); od[:4] = [0, 31, 1 << 23, (1 << 24) - 1]
+    for seed in (0, 1234, (1 << 64) - 1):
+        out = np.zeros((n, 3), np.float32)
+        dev.dev_vertex_jitter.argtypes = [C.c_uint64, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), f32p]
+        assert dev.dev_vertex_jitter(seed, n, si.ctypes.data_as(C.POINTER(C.c_uint64)), od.ctypes.data_as(C.POINTER(C.c_uint32)), out.ctypes.data_as(f32p)) == 0
+        want = np.array([_pcg_vertex_jitter(seed, int(s), int(o)) for s, o in zip(si, od)], np.float32)
+        assert np.array_equal(out.view(np.uint32), want.view(np.uint32)), seed
+        assert ((out >= 0) & (out < 1)).all() and len(np.unique(out)) > 2 * n
