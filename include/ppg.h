@@ -400,11 +400,11 @@ int ppg_op_dtree_pdf(int device,
 
 /* DTreeWrapper::sample (GP:619-621 -> 431-442, 257-301) with REPLAYED uniforms:
  * rnd holds rnd_stride floats per query, consumed in the reference's order (one per level, two at the leaf).
- * dir_out: 3 floats per query. */
+ * dir_out: 3 floats per query.  canonical_out (2 floats per query, or NULL): the point DTree::sample returns, before canonicalToDir. */
 int ppg_op_dtree_sample(int device,
                         const float *sums, const uint16_t *children, size_t n_nodes,
                         const uint32_t *tree_first_node, const float *tree_sum, const float *tree_weight, size_t n_trees,
-                        const uint32_t *query_tree, const float *rnd, size_t rnd_stride, size_t n, float *dir_out);
+                        const uint32_t *query_tree, const float *rnd, size_t rnd_stride, size_t n, float *dir_out, float *canonical_out);
 
 /* DTreeWrapper::record (GP:575-584 -> 395-413, 303-338) for n records into the
  * building sums (in/out) and per-tree statistical weights (in/out); filter = ppg_directional_filter. */

@@ -30,6 +30,7 @@ struct PortBackend {
     float bsdfSamplingFraction(Leaf *l) const { return l->dTree.bsdfSamplingFraction(); }
     void sample(Leaf *l, Pcg32 &rng, float *dir) const { PortRng r{rng}; V3 d = l->dTree.sample(r); dir[0] = d.x; dir[1] = d.y; dir[2] = d.z; }
     void sampleReplay(Leaf *l, const float *rnd, size_t n, float *dir) const { ReplayRng r{rnd, n}; V3 d = l->dTree.sample(r); dir[0] = d.x; dir[1] = d.y; dir[2] = d.z; }
+    void sampleCanonicalReplay(Leaf *l, const float *rnd, size_t n, float *p) const { ReplayRng r{rnd, n}; V2 c = l->dTree.sampling.sample(r); p[0] = c.x; p[1] = c.y; }
     float pdf(Leaf *l, const float *d) const { return l->dTree.pdf(V3{d[0], d[1], d[2]}); }
 
     // the spatial-filter switch of Vertex::commit, GP:1742-1767

@@ -323,6 +323,11 @@ int ppgo_tree_sample(ppgo_handle *h, size_t n, const uint32_t *leaf, const float
     for (size_t i = 0; i < n; ++i) T.sampleReplay(T.leafAt(leaf[i]), rnd + rnd_stride * i, rnd_stride, dir_out + 3 * i);
     return PPG_OK;
 }
+int ppgo_tree_sample_canonical(ppgo_handle *h, size_t n, const uint32_t *leaf, const float *rnd, size_t rnd_stride, float *point_out) {
+    BackendT &T = h->T();
+    for (size_t i = 0; i < n; ++i) T.sampleCanonicalReplay(T.leafAt(leaf[i]), rnd + rnd_stride * i, rnd_stride, point_out + 2 * i);
+    return PPG_OK;
+}
 int ppgo_tree_fraction(ppgo_handle *h, size_t n, const uint32_t *leaf, float *frac_out) {
     BackendT &T = h->T();
     for (size_t i = 0; i < n; ++i) frac_out[i] = T.bsdfSamplingFraction(T.leafAt(leaf[i]));

@@ -77,6 +77,8 @@ int ppgo_tree_record(ppgo_handle *h, size_t n, const float *o, const float *d, c
 int ppgo_tree_lookup(ppgo_handle *h, size_t n, const float *p, uint32_t *leaf_out, float *size_out);
 int ppgo_tree_pdf(ppgo_handle *h, size_t n, const uint32_t *leaf, const float *dir, float *pdf_out);
 int ppgo_tree_sample(ppgo_handle *h, size_t n, const uint32_t *leaf, const float *rnd, size_t rnd_stride, float *dir_out);
+/* the sampling D-tree's DTree::sample (GP:431-442) with the same replayed uniforms: the point in [0,1]^2 before canonicalToDir, 2 floats per query */
+int ppgo_tree_sample_canonical(ppgo_handle *h, size_t n, const uint32_t *leaf, const float *rnd, size_t rnd_stride, float *point_out);
 int ppgo_tree_fraction(ppgo_handle *h, size_t n, const uint32_t *leaf, float *frac_out);
 /* counts[0]=S-tree nodes, [1]=leaves, [2]=total sampling quadtree nodes, [3]=total building quadtree nodes */
 int ppgo_tree_counts(ppgo_handle *h, uint64_t counts[4]);

@@ -30,6 +30,7 @@ struct RefBackend {
     float bsdfSamplingFraction(Leaf *l) const { return l->bsdfSamplingFraction(); }
     void sample(Leaf *l, Pcg32 &rng, float *dir) const { RefSampler s; s.r = &rng; mitsuba::Vector d = l->sample(&s); dir[0] = d.x; dir[1] = d.y; dir[2] = d.z; }
     void sampleReplay(Leaf *l, const float *rnd, size_t n, float *dir) const { RefSampler s; s.v = rnd; s.n = n; mitsuba::Vector d = l->sample(&s); dir[0] = d.x; dir[1] = d.y; dir[2] = d.z; }
+    void sampleCanonicalReplay(Leaf *l, const float *rnd, size_t n, float *p) const { RefSampler s; s.v = rnd; s.n = n; mitsuba::Point2 c = l->sampling.sample(&s); p[0] = c.x; p[1] = c.y; }
     float pdf(Leaf *l, const float *d) const { return l->pdf(mitsuba::Vector(d[0], d[1], d[2])); }
 
     // the spatial-filter switch of Vertex::commit (GP:1742-1767 lies outside the verbatim extract, so it is restated here)

@@ -567,7 +567,7 @@ static int init_tree(ppg_integrator *h) {
 
 static TreeView tree_view(ppg_integrator *h) {
     TreeView T;
-    T.snodes = h->dSnodes.p; T.stable = h->dStable.p; T.leafA = h->dLeafA.p; T.samp = h->dSamp.p; T.bchildren = h->dBchildren.p;
+    T.snodes = h->dSnodes.p; T.stable = stree_table_usable(h->hNodes) ? h->dStable.p : nullptr; T.leafA = h->dLeafA.p; T.samp = h->dSamp.p; T.bchildren = h->dBchildren.p;
     T.bsums = reinterpret_cast<float4 *>(h->dTrain.p); T.bweight = h->dBweight.p;
     T.aabbMin = make_float3(h->aabbMin[0], h->aabbMin[1], h->aabbMin[2]); T.extent = make_float3(h->extent[0], h->extent[1], h->extent[2]);
     return T;
@@ -616,9 +616,12 @@ static int reset_sd_tree(ppg_integrator *h) {
     dtree_reset_kernel<true><<<blocks, 128, 0, h->stream>>>(M, h->dBuildBase.p, 20, h->prm.d_tree_threshold); h->launches++;
     leaf_after_reset_kernel<<<blocks, 256, 0, h->stream>>>(M, h->dBuildBase.p); h->launches++;
     h->toc();
-    // prefix table of the refined S-tree (stree_lookup): the first 3 * PPG_STREE_TABLE_BITS levels of every descent become one load
-    CK(h->dStable.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-    h->tic(PPG_K_REFINE); stree_table_kernel<<<h->numSMs * 8, 256, 0, h->stream>>>(h->dSnodes.p, h->dStable.p); h->toc(); h->launches++;
+    // prefix table of the refined S-tree (stree_lookup): the first 3 * PPG_STREE_TABLE_BITS levels of every descent become one load.
+    // Past 0xFFFFFF nodes its entries cannot hold the node numbers: tree_view then hands out no table and the kernels walk from the root.
+    if (stree_table_usable(h->hNodes)) {
+        CK(h->dStable.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
+        h->tic(PPG_K_REFINE); stree_table_kernel<<<h->numSMs * 8, 256, 0, h->stream>>>(h->dSnodes.p, h->dStable.p); h->toc(); h->launches++;
+    }
     CK(cudaGetLastError());
     return PPG_OK;      // no synchronize: the passes queue behind the reset
 }
@@ -1244,13 +1247,16 @@ __global__ void op_pdf_kernel(const SampNode *pool, const uint32_t *first, const
         out[i] = dtree_pdf(pool + first[t], mean > 0.f, dir_to_canonical(f3(qd[3 * i], qd[3 * i + 1], qd[3 * i + 2])));
     }
 }
-__global__ void op_sample_kernel(const SampNode *pool, const uint32_t *first, const float *tsum, const float *tweight, const uint32_t *qt, const float *rnd, size_t stride, size_t n, float *out) {
+__global__ void op_sample_kernel(const SampNode *pool, const uint32_t *first, const float *tsum, const float *tweight, const uint32_t *qt, const float *rnd, size_t stride, size_t n, float *out,
+                                 float *canon) {
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
         const uint32_t t = qt[i];
         float mean = 0.f; if (tweight[t] != 0.f) mean = (1.f / (PPG_PI * 4.f * tweight[t])) * tsum[t];
         ReplayRng r{rnd + stride * i, (uint32_t) stride, 0u};
-        const float3 d = canonical_to_dir(dtree_sample(pool + first[t], mean > 0.f, r));
+        const float2 c = dtree_sample(pool + first[t], mean > 0.f, r);
+        const float3 d = canonical_to_dir(c);
         out[3 * i] = d.x; out[3 * i + 1] = d.y; out[3 * i + 2] = d.z;
+        if (canon) { canon[2 * i] = c.x; canon[2 * i + 1] = c.y; }
     }
 }
 __global__ void op_record_kernel(const __grid_constant__ TreeView T, const uint32_t *rt, const float *rd, const float *rrad, const float *rpdf, const float *rw, size_t n, int filter) {
@@ -1335,16 +1341,18 @@ extern "C" int ppg_op_dtree_pdf(int device, const float *sums, const uint16_t *c
 }
 extern "C" int ppg_op_dtree_sample(int device, const float *sums, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
                                    const float *tree_sum, const float *tree_weight, size_t n_trees, const uint32_t *query_tree, const float *rnd,
-                                   size_t rnd_stride, size_t n, float *dir_out) {
+                                   size_t rnd_stride, size_t n, float *dir_out, float *canonical_out) {
     int rc = op_device(device); if (rc) return rc;
     std::vector<SampNode> pool = to_pool(sums, children, n_nodes);
-    Up<SampNode> dp; Up<uint32_t> df, dq; Up<float> ds, dw, dr; DevBuf<float> out;
+    Up<SampNode> dp; Up<uint32_t> df, dq; Up<float> ds, dw, dr; DevBuf<float> out, canon;
     if (dp.up(pool.data(), n_nodes) || df.up(tree_first_node, n_trees) || ds.up(tree_sum, n_trees) || dw.up(tree_weight, n_trees) || dq.up(query_tree, n) || dr.up(rnd, rnd_stride * n))
         return fail(PPG_ERR_CUDA, "upload failed");
     CK(out.alloc(std::max<size_t>(3 * n, 1)));
-    if (n) op_sample_kernel<<<296, 256>>>(dp.b.p, df.b.p, ds.b.p, dw.b.p, dq.b.p, dr.b.p, rnd_stride, n, out.p);
+    if (canonical_out) CK(canon.alloc(std::max<size_t>(2 * n, 1)));
+    if (n) op_sample_kernel<<<296, 256>>>(dp.b.p, df.b.p, ds.b.p, dw.b.p, dq.b.p, dr.b.p, rnd_stride, n, out.p, canon.p);
     CK(cudaGetLastError());
     CK(cudaMemcpy(dir_out, out.p, 12 * n, cudaMemcpyDeviceToHost));
+    if (canonical_out) CK(cudaMemcpy(canonical_out, canon.p, 8 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
 }
 extern "C" int ppg_op_dtree_record(int device, float *sums_inout, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
@@ -1420,9 +1428,12 @@ extern "C" int ppg_op_stree_lookup(int device, const uint32_t *node_children, si
     Up<uint2> dn; Up<float> dp; DevBuf<uint32_t> dl; DevBuf<float> dsz;
     if (dn.up(reinterpret_cast<const uint2 *>(node_children), n_nodes) || dp.up(points, 3 * n)) return fail(PPG_ERR_CUDA, "upload failed");
     CK(dl.alloc(std::max<size_t>(n, 1))); CK(dsz.alloc(std::max<size_t>(3 * n, 1)));
-    DevBuf<uint32_t> dt; CK(dt.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-    stree_table_kernel<<<296, 256>>>(dn.b.p, dt.p);     // the same prefix table the render kernels use
-    if (n) op_lookup_kernel<<<296, 256>>>(dn.b.p, dt.p, make_float3(aabb_min[0], aabb_min[1], aabb_min[2]), make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]), dp.b.p, n, dl.p, dsz.p);
+    DevBuf<uint32_t> dt;
+    if (stree_table_usable(n_nodes)) {                    // the same prefix table the render kernels use, under the same rule
+        CK(dt.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
+        stree_table_kernel<<<296, 256>>>(dn.b.p, dt.p);
+    }
+    if (n) op_lookup_kernel<<<296, 256>>>(dn.b.p, dt.p,make_float3(aabb_min[0], aabb_min[1], aabb_min[2]), make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]), dp.b.p, n, dl.p, dsz.p);
     CK(cudaGetLastError());
     CK(cudaMemcpy(leaf_out, dl.p, 4 * n, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(size_out, dsz.p, 12 * n, cudaMemcpyDeviceToHost));
@@ -1583,8 +1594,10 @@ extern "C" int ppg_op_commit(int device, int record_mode, const uint32_t *node_c
     CK(dev_array(dBch, n_pool, reinterpret_cast<const uint2 *>(children), n_pool)); CK(dev_array(dBs, n_pool, reinterpret_cast<const float4 *>(sums_inout), n_pool));
     CK(dev_array(dSlab, slab.size(), slab.data(), slab.size())); CK(dev_array(dLi, n_li, reinterpret_cast<const float4 *>(li_final), n_li));
     CK(dev_array(dLive, 1, &live, 1)); CK(dev_array(dTot, 1)); CK(dev_array(dDrop, 1)); CK(dev_array(dRA, cap)); CK(dev_array(dRB, cap));
-    CK(dev_array(dTab, (size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-    stree_table_kernel<<<296, 256>>>(dS.p, dTab.p);        // as after every refine (reset_sd_tree)
+    if (stree_table_usable(n_nodes)) {                      // as after every refine (reset_sd_tree)
+        CK(dev_array(dTab, (size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
+        stree_table_kernel<<<296, 256>>>(dS.p, dTab.p);
+    }
     CommitParams C; memset(&C, 0, sizeof(C));
     C.tree.snodes = dS.p; C.tree.stable = dTab.p; C.tree.leafA = dLA.p; C.tree.samp = nullptr; C.tree.bchildren = dBch.p; C.tree.bsums = dBs.p; C.tree.bweight = dBW.p;
     C.tree.aabbMin = make_float3(aabb_min[0], aabb_min[1], aabb_min[2]); C.tree.extent = make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]);

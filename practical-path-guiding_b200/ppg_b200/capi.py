@@ -218,7 +218,7 @@ def load_library(path: str | None = None):
     lib.ppg_get_moment_images.argtypes = [H, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     u16p = C.POINTER(C.c_uint16); u32p = C.POINTER(C.c_uint32); f32p = C.POINTER(C.c_float)
     lib.ppg_op_dtree_pdf.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, f32p, C.c_size_t, u32p, f32p, C.c_size_t, f32p]
-    lib.ppg_op_dtree_sample.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, f32p, C.c_size_t, u32p, f32p, C.c_size_t, C.c_size_t, f32p]
+    lib.ppg_op_dtree_sample.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, f32p, C.c_size_t, u32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p]
     lib.ppg_op_dtree_record.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, C.c_size_t, u32p, f32p, f32p, f32p, f32p, C.c_size_t, C.c_int]
     lib.ppg_op_stree_lookup.argtypes = [C.c_int, u32p, C.c_size_t, f32p, f32p, f32p, C.c_size_t, u32p, f32p]
     lib.ppg_op_bvh_build.argtypes = [f32p, u32p, C.c_size_t, C.c_int, f32p, C.c_size_t, u32p, C.POINTER(C.c_size_t), C.POINTER(C.c_int), C.POINTER(C.c_double)]

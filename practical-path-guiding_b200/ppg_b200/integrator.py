@@ -208,15 +208,18 @@ def op_dtree_pdf(sums, children, tree_first, tree_sum, tree_weight, query_tree, 
     return out
 
 
-def op_dtree_sample(sums, children, tree_first, tree_sum, tree_weight, query_tree, rnd, device=0):
+def op_dtree_sample(sums, children, tree_first, tree_sum, tree_weight, query_tree, rnd, device=0, canonical=False):
+    """Sampled directions (n, 3); with canonical=True also the points DTree::sample returns before canonicalToDir, (n, 2)."""
     lib = capi.load_library()
     sums = np.ascontiguousarray(sums, np.float32); children = np.ascontiguousarray(children, np.uint16)
     tf = np.ascontiguousarray(tree_first, np.uint32); ts = np.ascontiguousarray(tree_sum, np.float32); tw = np.ascontiguousarray(tree_weight, np.float32)
     qt = np.ascontiguousarray(query_tree, np.uint32); rnd = np.ascontiguousarray(rnd, np.float32)
     out = np.zeros((len(qt), 3), np.float32)
+    canon = np.zeros((len(qt), 2), np.float32) if canonical else None
     _check(lib, lib.ppg_op_dtree_sample(device, _p(sums, C.c_float), _p(children, C.c_uint16), len(sums), _p(tf, C.c_uint32), _p(ts, C.c_float),
-                                        _p(tw, C.c_float), len(tf), _p(qt, C.c_uint32), _p(rnd, C.c_float), rnd.shape[1], len(qt), _p(out, C.c_float)))
-    return out
+                                        _p(tw, C.c_float), len(tf), _p(qt, C.c_uint32), _p(rnd, C.c_float), rnd.shape[1], len(qt), _p(out, C.c_float),
+                                        None if canon is None else _p(canon, C.c_float)))
+    return (out, canon) if canonical else out
 
 
 def op_dtree_record(sums, children, tree_first, tree_weight, rec_tree, rec_dir, rec_radiance, rec_wo_pdf, rec_weight, directional_filter=0, device=0):

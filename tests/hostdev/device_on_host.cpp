@@ -119,18 +119,19 @@ int dev_discrete(size_t n_entries, const float *cdf, size_t n, const float *samp
 int dev_stree_lookup(const uint32_t *node_children /* 2 per node */, size_t n_nodes, const float aabb_min[3], const float extent[3], const float *points, size_t n, uint32_t *leaf_out, float *size_out) {
     std::vector<uint2> sn(n_nodes);
     for (size_t i = 0; i < n_nodes; ++i) sn[i] = make_uint2(node_children[2 * i], node_children[2 * i + 1]);
-    std::vector<uint32_t> table((size_t) 1 << (3 * PPG_STREE_TABLE_BITS));
-    stree_table_kernel(sn.data(), table.data());
+    std::vector<uint32_t> table;                     // under the render's rule: no table past 0xFFFFFF nodes
+    if (stree_table_usable(n_nodes)) { table.resize((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)); stree_table_kernel(sn.data(), table.data()); }
     const float3 mn = make_float3(aabb_min[0], aabb_min[1], aabb_min[2]), ex = make_float3(extent[0], extent[1], extent[2]);
     for (size_t i = 0; i < n; ++i) {
-        int lv = 0; leaf_out[i] = stree_lookup(sn.data(), table.data(), mn, ex, v3(points, i), lv);
+        int lv = 0; leaf_out[i] = stree_lookup(sn.data(), table.empty() ? nullptr : table.data(), mn, ex, v3(points, i), lv);
         const float3 v = voxel_size(ex, lv); size_out[3 * i] = v.x; size_out[3 * i + 1] = v.y; size_out[3 * i + 2] = v.z;
     }
     return 0;
 }
 struct ReplayRng { const float *v; uint32_t n, i; float next1D() { return i < n ? v[i++] : 0.5f; } };
 int dev_dtree(const float *sums, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first, const float *tree_sum, const float *tree_weight,
-              const uint32_t *query_tree, const float *query_dir, const float *rnd, size_t rnd_stride, size_t n, float *pdf_out, float *dir_out) {
+              const uint32_t *query_tree, const float *query_dir, const float *rnd, size_t rnd_stride, size_t n, float *pdf_out, float *dir_out,
+              float *canonical_out /* 2n or NULL: the point dtree_sample returns, before canonical_to_dir */) {
     std::vector<SampNode> pool(n_nodes);
     for (size_t i = 0; i < n_nodes; ++i) {
         pool[i].sums = make_float4(sums[4 * i], sums[4 * i + 1], sums[4 * i + 2], sums[4 * i + 3]);
@@ -142,8 +143,10 @@ int dev_dtree(const float *sums, const uint16_t *children, size_t n_nodes, const
         float mean = 0.f; if (tree_weight[t] != 0.f) mean = (1.f / (PPG_PI * 4.f * tree_weight[t])) * tree_sum[t];       // DTree::mean, GP:386-394
         pdf_out[i] = dtree_pdf(pool.data() + tree_first[t], mean > 0.f, dir_to_canonical(v3(query_dir, i)));
         ReplayRng r{rnd + rnd_stride * i, (uint32_t) rnd_stride, 0u};
-        const float3 d = canonical_to_dir(dtree_sample(pool.data() + tree_first[t], mean > 0.f, r));
+        const float2 c = dtree_sample(pool.data() + tree_first[t], mean > 0.f, r);
+        const float3 d = canonical_to_dir(c);
         dir_out[3 * i] = d.x; dir_out[3 * i + 1] = d.y; dir_out[3 * i + 2] = d.z;
+        if (canonical_out) { canonical_out[2 * i] = c.x; canonical_out[2 * i + 1] = c.y; }
     }
     return 0;
 }

@@ -50,6 +50,8 @@ def _declare(lib):
     lib.ppgo_tree_lookup.argtypes = [H, C.c_size_t, f32p, u32p, f32p]
     lib.ppgo_tree_pdf.argtypes = [H, C.c_size_t, u32p, f32p, f32p]
     lib.ppgo_tree_sample.argtypes = [H, C.c_size_t, u32p, f32p, C.c_size_t, f32p]
+    if hasattr(lib, "ppgo_tree_sample_canonical"):     # a reference library built by an older oracle/Makefile recipe lacks it
+        lib.ppgo_tree_sample_canonical.argtypes = [H, C.c_size_t, u32p, f32p, C.c_size_t, f32p]
     lib.ppgo_tree_fraction.argtypes = [H, C.c_size_t, u32p, f32p]
     lib.ppgo_tree_counts.argtypes = [H, u64p]
     lib.ppgo_tree_export.argtypes = [H, C.c_int, u32p, i32p, u8p, u64p, u32p, f32p, f32p, i32p, f32p, u16p, f32p, f32p]
@@ -265,6 +267,17 @@ class Oracle:
         leaf = np.ascontiguousarray(leaf, np.uint32); rnd = np.ascontiguousarray(rnd, np.float32)
         out = np.zeros((len(leaf), 3), np.float32)
         self.lib.ppgo_tree_sample(self.h, len(leaf), leaf.ctypes.data_as(C.POINTER(C.c_uint32)), fptr(rnd), rnd.shape[1], fptr(out))
+        return out
+
+    def has_sample_canonical(self):
+        """Whether the loaded library has ppgo_tree_sample_canonical (the library built from this tree's oracle/ always has it)."""
+        return hasattr(self.lib, "ppgo_tree_sample_canonical")
+
+    def sample_canonical(self, leaf, rnd):
+        """DTree::sample of the leaves' sampling trees with replayed uniforms: the point in [0,1]^2 before canonicalToDir, (n, 2)."""
+        leaf = np.ascontiguousarray(leaf, np.uint32); rnd = np.ascontiguousarray(rnd, np.float32)
+        out = np.zeros((len(leaf), 2), np.float32)
+        self.lib.ppgo_tree_sample_canonical(self.h, len(leaf), leaf.ctypes.data_as(C.POINTER(C.c_uint32)), fptr(rnd), rnd.shape[1], fptr(out))
         return out
 
     def fraction(self, leaf):

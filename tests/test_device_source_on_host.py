@@ -287,9 +287,9 @@ def test_device_sdtree_sources_against_the_reference_trees(dev):
     rnd = rng.random((n, 24), dtype=np.float32)
     pdf = np.zeros(n, np.float32); dirs = np.zeros((n, 3), np.float32)
     sums = np.ascontiguousarray(e["sums"], np.float32); ch = np.ascontiguousarray(e["children"], np.uint16); first = e["tree_first"].astype(np.uint32)
-    dev.dev_dtree.argtypes = [f32p, C.POINTER(C.c_uint16), C.c_size_t, u32p, f32p, f32p, u32p, f32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p]
+    dev.dev_dtree.argtypes = [f32p, C.POINTER(C.c_uint16), C.c_size_t, u32p, f32p, f32p, u32p, f32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p, f32p]
     dev.dev_dtree(sums.ctypes.data_as(f32p), ch.ctypes.data_as(C.POINTER(C.c_uint16)), len(sums), first.ctypes.data_as(u32p), e["tree_sum"].ctypes.data_as(f32p),
-                  e["tree_weight"].ctypes.data_as(f32p), ql.ctypes.data_as(u32p), d.ctypes.data_as(f32p), rnd.ctypes.data_as(f32p), 24, n, pdf.ctypes.data_as(f32p), dirs.ctypes.data_as(f32p))
+                  e["tree_weight"].ctypes.data_as(f32p), ql.ctypes.data_as(u32p), d.ctypes.data_as(f32p), rnd.ctypes.data_as(f32p), 24, n, pdf.ctypes.data_as(f32p), dirs.ctypes.data_as(f32p), None)
     ref_pdf = o.pdf(ql, d); ref_dir = o.sample(ql, rnd)
     assert np.allclose(pdf, ref_pdf, rtol=2e-6, atol=1e-12) and np.abs(dirs - ref_dir).max() <= 2e-6
     assert (dirs == ref_dir).all(axis=1).mean() > 0.9                              # (mostly bit-equal: same libm here)
@@ -472,3 +472,102 @@ def test_vertex_jitter_source_is_pcg32_of_the_vertex_stream(dev):
         want = np.array([_pcg_vertex_jitter(seed, int(s), int(o)) for s, o in zip(si, od)], np.float32)
         assert np.array_equal(out.view(np.uint32), want.view(np.uint32)), seed
         assert ((out >= 0) & (out < 1)).all() and len(np.unique(out)) > 2 * n
+
+
+# ---- the query half of the SD-tree at the depths the render reaches (tests/sdtree_queries.py; the same cases run on the GPU in tests/test_gpu_sdtree_queries.py)
+def _dev_lookup(dev, sch, mn, ext, pts):
+    u32p = C.POINTER(C.c_uint32)
+    sch = np.ascontiguousarray(sch, np.uint32); pts = np.ascontiguousarray(pts, np.float32)
+    mn = np.ascontiguousarray(mn, np.float32); ext = np.ascontiguousarray(ext, np.float32)
+    leaf = np.zeros(len(pts), np.uint32); size = np.zeros((len(pts), 3), np.float32)
+    dev.dev_stree_lookup.argtypes = [u32p, C.c_size_t, f32p, f32p, f32p, C.c_size_t, u32p, f32p]
+    assert dev.dev_stree_lookup(sch.ctypes.data_as(u32p), len(sch), mn.ctypes.data_as(f32p), ext.ctypes.data_as(f32p), pts.ctypes.data_as(f32p), len(pts),
+                                leaf.ctypes.data_as(u32p), size.ctypes.data_as(f32p)) == 0
+    return leaf, size
+
+
+def _cbox_box():
+    from common import load_cbox
+    o = O.Oracle(O.default_params(), load_cbox(16), kind="port")
+    mn, mx = o.export(0)["aabb"]; o.close()
+    return mn.astype(np.float32), mx.astype(np.float32)
+
+
+@pytest.mark.parametrize("box", ["dyadic", "cbox"])
+def test_device_stree_lookup_at_the_prefix_table_boundary(dev, box):
+    """stree_lookup on a synthetic S-tree with leaves at exactly 20, 21 and 22 levels (the prefix table resolves 21), in a power-of-two box and in
+    the cubified CBOX box: uniform points, points exactly on the split planes of every inner node from depth 15 down and of up to 24 levels per axis
+    around the deep leaves, points on the faces and one ulp inside / outside them, points far outside.  Leaf and voxel size equal the float32 walk of
+    the reference bit for bit."""
+    import sdtree_queries as Q
+    mn, mx = Q.DYADIC_BOX if box == "dyadic" else _cbox_box()
+    ext = (mx - mn).astype(np.float32)
+    sch = Q.synthetic_stree(Q.SYNTHETIC_ANCHORS)
+    rng = np.random.default_rng(31)
+    pts = np.concatenate([Q.stree_points(rng, mn, ext, [a for a, _ in Q.SYNTHETIC_ANCHORS]), Q.split_plane_points(sch, mn, ext, 15)])
+    wl, ws, wd = Q.stree_walk(sch, mn, ext, pts)
+    assert {20, 21, 22} <= set(wd.tolist())
+    gl, gs = _dev_lookup(dev, sch, mn, ext, pts)
+    assert np.array_equal(gl, wl) and np.array_equal(gs.view(np.uint32), ws.view(np.uint32))
+
+
+def test_device_stree_lookup_past_2to24_nodes(dev):
+    """The synthetic tree above renumbered so that every node but the root carries a number >= 2^24 (2^24 + 5 unreachable leaves in between, the
+    layout later refines produce): the table's 24-bit node field cannot hold them, so the lookup walks from the root -- leaves bit for bit."""
+    import sdtree_queries as Q
+    mn, mx = Q.DYADIC_BOX; ext = (mx - mn).astype(np.float32)
+    sch = Q.synthetic_stree(Q.SYNTHETIC_ANCHORS, offset=(1 << 24) + 5)
+    rng = np.random.default_rng(32)
+    pts = np.concatenate([Q.stree_points(rng, mn, ext, [a for a, _ in Q.SYNTHETIC_ANCHORS], 5000), Q.split_plane_points(sch, mn, ext, 15)])
+    wl, ws, wd = Q.stree_walk(sch, mn, ext, pts)
+    assert len(sch) > 1 << 24 and (wl >= 1 << 24).all() and {20, 21, 22} <= set(wd.tolist())
+    gl, gs = _dev_lookup(dev, sch, mn, ext, pts)
+    assert np.array_equal(gl, wl), f"{int((gl != wl).sum())} of {len(wl)} leaves differ, e.g. {gl[gl != wl][:4]} for {wl[gl != wl][:4]}"
+    assert np.array_equal(gs.view(np.uint32), ws.view(np.uint32))
+
+
+@pytest.fixture(scope="module")
+def dtrees():
+    import sdtree_queries as Q
+    return Q.dtree_trees(O, "ref" if O.have_ref() else "port")
+
+
+def _dev_dtree(dev, e, ql, d, rnd):
+    u32p = C.POINTER(C.c_uint32)
+    n = len(ql); pdf = np.zeros(n, np.float32); dirs = np.zeros((n, 3), np.float32); canon = np.zeros((n, 2), np.float32)
+    sums = np.ascontiguousarray(e["sums"], np.float32); ch = np.ascontiguousarray(e["children"], np.uint16); first = e["tree_first"].astype(np.uint32)
+    ql = np.ascontiguousarray(ql, np.uint32); d = np.ascontiguousarray(d, np.float32); rnd = np.ascontiguousarray(rnd, np.float32)
+    dev.dev_dtree.argtypes = [f32p, C.POINTER(C.c_uint16), C.c_size_t, u32p, f32p, f32p, u32p, f32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p, f32p]
+    dev.dev_dtree(sums.ctypes.data_as(f32p), ch.ctypes.data_as(C.POINTER(C.c_uint16)), len(sums), first.ctypes.data_as(u32p), e["tree_sum"].ctypes.data_as(f32p),
+                  e["tree_weight"].ctypes.data_as(f32p), ql.ctypes.data_as(u32p), d.ctypes.data_as(f32p), rnd.ctypes.data_as(f32p), rnd.shape[1], n,
+                  pdf.ctypes.data_as(f32p), dirs.ctypes.data_as(f32p), canon.ctypes.data_as(f32p))
+    return pdf, dirs, canon
+
+
+def test_device_dtree_queries_at_the_depth_cap(dev, dtrees):
+    """dtree_pdf and dtree_sample on the oracle's depth-20 cone trees, the 65 536-node tree and an untrained tree (tests/sdtree_queries.dtree_trees).
+    pdf at random directions, the poles, the phi seam, canonical points on quadrant boundaries of every level and inside zero-sum cells: zeros exact,
+    elsewhere within (5 * depth + 2) * 2^-24 of the float64 product of the exact ratios (the oracle's pdf too).  Samples with random, extreme and
+    boundary uniforms: the canonical point bit-equal to the float32 restatement and to the reference's DTree::sample point; directions within 2e-6."""
+    import sdtree_queries as Q
+    o, e, leaves, cones = dtrees
+    rng = np.random.default_rng(33)
+    first = e["tree_first"].astype(np.int64); valid = Q.valid_flags(e["tree_sum"], e["tree_weight"])
+    ql, d, ex = [], [], []
+    for k, leaf in enumerate(leaves):
+        dk, exk = Q.pdf_directions(rng, e["sums"], e["children"], int(first[leaf]), cones[k])
+        ql.append(np.full(len(dk), leaf, np.uint32)); d.append(dk); ex.append(exk)
+    ql, d, ex = np.concatenate(ql), np.concatenate(d), np.concatenate(ex)
+    rnd = Q.sample_uniforms(rng, e["sums"], e["children"], first[ql], valid[ql], len(ql))
+    pdf, dirs, canon = _dev_dtree(dev, e, ql, d, rnd)
+    ok, depth = Q.pdf_matches(pdf, e["sums"], e["children"], first[ql], valid[ql], d, exact_phi=ex)
+    assert ok.all(), (np.nonzero(~ok)[0][:8], pdf[~ok][:8])
+    ok_o, _ = Q.pdf_matches(o.pdf(ql, d), e["sums"], e["children"], first[ql], valid[ql], d, exact_phi=ex)
+    assert ok_o.all()
+    assert depth.max() == 20 and (pdf == 0).any() and (pdf[~valid[ql]] == np.float32(1) / (np.float32(4) * Q.PI32)).all()
+    want, levels = Q.sample_reference(e["sums"], e["children"], first[ql], valid[ql], rnd)
+    assert np.array_equal(canon.view(np.uint32), want.view(np.uint32)), int((canon != want).any(axis=1).sum())
+    assert o.has_sample_canonical() or o.kind == "ref"          # (a prebuilt reference library may predate the entry)
+    if o.has_sample_canonical():
+        assert np.array_equal(canon.view(np.uint32), o.sample_canonical(ql, rnd).view(np.uint32))
+    assert np.abs(dirs - o.sample(ql, rnd)).max() <= 2e-6 and levels.max() == 20
