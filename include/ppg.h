@@ -368,6 +368,19 @@ int ppg_cancel(ppg_integrator *h);
 /* dumpSDTree wire format (GP:1191-1208, 699-711, 945-951), current sampling trees. */
 int ppg_dump_sdtree(ppg_integrator *h, const char *path);
 
+/* The integrator's SD-tree as flat host arrays, after ppg_render or from inside the film callback (after an iteration's passes, before its
+ * build: the S-tree is refined, the sampling trees are the ones the passes guided with, the building trees hold what they recorded).
+ * which: 0 = sampling trees, 1 = building trees.  Per S-tree node, in the integrator's own numbering: node_children (2 x u32, 0 0 for a leaf),
+ * tree_first (u64 offset of the node's quadtree in sums / children), tree_count, tree_depth, tree_sum, tree_weight (sampling: the tree's sum and
+ * statistical weight; building: sum 0 and the weight recorded so far), adam (6 floats: iter, m, v, theta as the bounce kernel reads it,
+ * batchAcc, batchGrad).  Inner nodes carry zeros.  The quadtrees of the leaves, concatenated in node order: sums (4 floats) and children
+ * (4 x u16) per quadtree node.  aabb_min_max: the cubified S-tree box (6 floats).  Output arrays hold node_capacity nodes and pool_capacity
+ * quadtree nodes; if either is too small the call returns PPG_ERR_INVALID_ARGUMENT with *n_nodes_out and *n_pool_out set to the sizes
+ * needed.  Output pointers other than the counts may be NULL. */
+int ppg_export_sdtree(ppg_integrator *h, int which, size_t node_capacity, size_t *n_nodes_out, uint32_t *node_children, uint64_t *tree_first,
+                      uint32_t *tree_count, int32_t *tree_depth, float *tree_sum, float *tree_weight, float *adam,
+                      size_t pool_capacity, size_t *n_pool_out, float *sums, uint16_t *children, float *aabb_min_max);
+
 /* scene->getDestinationFile(): with dumpSDTree=true every non-final iteration writes "<destination>-NN.sdt"
  * (NN = two-digit iteration index, GP:1191-1195, 1417-1419). NULL/"" disables the per-iteration dumps. */
 int ppg_set_destination(ppg_integrator *h, const char *destination);

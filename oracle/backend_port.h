@@ -81,6 +81,47 @@ struct PortBackend {
     }
     void aabb(float *mn, float *mx) const { mn[0] = t.amin.x; mn[1] = t.amin.y; mn[2] = t.amin.z; mx[0] = t.amax.x; mx[1] = t.amax.y; mx[2] = t.amax.z; }
 
+    // the inverse of the sampling-side export (ppgo_tree_import): replaces the S-tree, keeps the box.  Node axes follow from the depth
+    // (x, y, z cycling from the root, GP:876-895); the building trees start empty (resetAll makes them).  false: not a valid tree.
+    bool importTree(size_t n, const uint32_t *sch, const uint64_t *first, const uint32_t *count, const float *sum, const float *weight, const int32_t *depth,
+                    const float *sums, const uint16_t *children, size_t nPool, const float *adam) {
+        if (n == 0 || n >= 0xFFFFFFFFull) return false;
+        std::vector<SNode> nodes(n);
+        std::vector<uint8_t> seen(n, 0);
+        std::vector<uint32_t> stack(1, 0u); seen[0] = 1;
+        while (!stack.empty()) {
+            const uint32_t i = stack.back(); stack.pop_back();
+            SNode &s = nodes[i];
+            if (sch[2 * i] != 0u || sch[2 * i + 1] != 0u) {
+                s.isLeaf = false;
+                for (int c = 0; c < 2; ++c) {
+                    const uint32_t k = sch[2 * i + c];
+                    if (k == 0u || k >= n || seen[k]) return false;
+                    seen[k] = 1; s.children[c] = k; nodes[k].axis = (s.axis + 1) % 3; stack.push_back(k);
+                }
+                s.dTree = DTreeWrapper();
+                continue;
+            }
+            const uint32_t cnt = count[i];
+            if (cnt == 0u || cnt > 65535u || first[i] > nPool || nPool - first[i] < cnt) return false;
+            DTree &d = s.dTree.sampling;
+            d.nodes.assign(cnt, QNode());
+            for (uint32_t k = 0; k < cnt; ++k)
+                for (int j = 0; j < 4; ++j) {
+                    d.nodes[k].sum[j] = sums[4 * (first[i] + k) + j];
+                    d.nodes[k].child[j] = children[4 * (first[i] + k) + j];
+                    if (d.nodes[k].child[j] >= cnt) return false;
+                }
+            d.sum = sum[i]; d.weight = weight[i]; d.maxDepth = depth[i];
+            Adam &a = s.dTree.opt;
+            const float *st = adam + 6 * (size_t) i;
+            a.iter = (int) st[0]; a.m1 = st[1]; a.m2 = st[2]; a.variable = st[3]; a.batchAcc = st[4]; a.batchGrad = st[5];
+        }
+        for (size_t i = 0; i < n; ++i) if (!seen[i]) return false;
+        t.nodes = std::move(nodes);
+        return true;
+    }
+
     // flat [building sums (4 per quadtree node) | building weight] per leaf in node order (the exchange buffer of SURVEY 8e)
     size_t packSize() const { size_t n = 0; for (const auto &nd : t.nodes) if (nd.isLeaf) n += 4 * nd.dTree.building.nodes.size() + 1; return n; }
     void packBuilding(float *buf, bool unpack) {

@@ -378,4 +378,24 @@ int ppgo_tree_export(ppgo_handle *h, int which, uint32_t *s_children, int32_t *s
     return PPG_OK;
 }
 
+int ppgo_tree_import(ppgo_handle *h, size_t n_nodes, const uint32_t *s_children, const uint64_t *tree_first, const uint32_t *tree_count,
+                     const float *tree_sum, const float *tree_weight, const int32_t *tree_depth, const float *sums, const uint16_t *children,
+                     size_t n_pool, const float *adam, int iter, int passes_rendered) {
+#ifdef PPGO_BACKEND_REF
+    (void) h; (void) n_nodes; (void) s_children; (void) tree_first; (void) tree_count; (void) tree_sum; (void) tree_weight; (void) tree_depth;
+    (void) sums; (void) children; (void) n_pool; (void) adam; (void) iter; (void) passes_rendered;
+    return PPG_ERR_UNSUPPORTED;
+#else
+    if (!s_children || !tree_first || !tree_count || !tree_sum || !tree_weight || !tree_depth || !sums || !children || !adam || iter < 0 || passes_rendered < 0)
+        return PPG_ERR_INVALID_ARGUMENT;
+    if (!h->T().importTree(n_nodes, s_children, tree_first, tree_count, tree_sum, tree_weight, tree_depth, sums, children, n_pool, adam)) return PPG_ERR_INVALID_ARGUMENT;
+    if (h->tracer) {
+        Tracer<BackendT> &t = *h->tracer;
+        t.iter = iter; t.passesRendered = passes_rendered; t.isBuilt = iter > 0;
+        t.doNee = t.doNeeWithSpp(passes_rendered * t.prm.spp_per_pass);
+    }
+    return PPG_OK;
+#endif
+}
+
 }  // extern "C"

@@ -89,6 +89,15 @@ int ppgo_tree_counts(ppgo_handle *h, uint64_t counts[4]);
 int ppgo_tree_export(ppgo_handle *h, int which, uint32_t *s_children, int32_t *s_axis, uint8_t *s_is_leaf,
                      uint64_t *tree_first, uint32_t *tree_count, float *tree_sum, float *tree_weight, int32_t *tree_depth,
                      float *sums, uint16_t *children, float *adam, float *aabb_min_max);
+/* import: replace the handle's S-tree by the arrays of a sampling-side export (any numbering; the box stays the handle's): s_children 2*N
+ * (0,0 for leaves), per leaf its sampling tree (tree_first / tree_count into sums / children, tree_sum, tree_weight, tree_depth) and per node
+ * the Adam state (6 floats).  Node axes follow from the depth.  The building trees are empty until ppgo_tree_reset.  With a scene the tracer
+ * then stands where the product stands after `passes_rendered` passes, at iteration `iter` (isBuilt = iter > 0, doNee from the spp rendered):
+ * the next ppgo_step_passes keys its paths like the product's next pass.  PPG_ERR_INVALID_ARGUMENT for arrays that are not a tree,
+ * PPG_ERR_UNSUPPORTED on the verbatim reference backend. */
+int ppgo_tree_import(ppgo_handle *h, size_t n_nodes, const uint32_t *s_children, const uint64_t *tree_first, const uint32_t *tree_count,
+                     const float *tree_sum, const float *tree_weight, const int32_t *tree_depth, const float *sums, const uint16_t *children,
+                     size_t n_pool, const float *adam, int iter, int passes_rendered);
 #ifdef __cplusplus
 }
 #endif

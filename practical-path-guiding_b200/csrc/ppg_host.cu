@@ -1180,6 +1180,83 @@ extern "C" int ppg_get_moment_images(ppg_integrator *h, float *sum_rgbw, float *
     return PPG_OK;
 }
 
+// The integrator's SD-tree on the host: the S-tree and, per node, either the sampling trees (which == 0: the trees the passes guide with) or the
+// building trees (which == 1: the trees the passes record into).  Between the reset and the build of an iteration (the film callback) the sampling
+// trees still sit where the previous build put them, past the new building total: the copy of the quadtree pool is sized from the leaves.
+struct TreeGather {
+    uint32_t n = 0;
+    std::vector<uint2> sn; std::vector<float4> la; std::vector<float> sum, weight, adam; std::vector<int> depth; std::vector<uint32_t> count;
+    std::vector<uint2> children; std::vector<float4> sums;      // the quadtree pool from offset 0 (building: bchildren / bsums; sampling: dSamp)
+    uint32_t first(uint32_t i, int which) const { uint32_t u; memcpy(&u, which ? &la[i].y : &la[i].x, 4); return u; }
+};
+static int gather_tree(ppg_integrator *h, int which, TreeGather &g) {
+    if (!h->haveScene || h->capNodes == 0) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
+    CK(cudaSetDevice(h->device));
+    const uint32_t n = g.n = h->hNodes;
+    g.sn.resize(n); g.la.resize(n); g.sum.assign(n, 0.f); g.weight.resize(n); g.adam.resize(6 * (size_t) n); g.depth.resize(n); g.count.resize(n);
+    CK(cudaMemcpy(g.sn.data(), h->dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g.la.data(), h->dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g.adam.data(), h->dAdam.p, 24 * (size_t) n, cudaMemcpyDeviceToHost));
+    if (which == 0) CK(cudaMemcpy(g.sum.data(), h->dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g.weight.data(), which ? h->dBweight.p : h->dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g.depth.data(), which ? h->dBuildDepth.p : h->dSampDepth.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g.count.data(), which ? h->dBuildCount.p : h->dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+    size_t end = 1;
+    for (uint32_t i = 0; i < n; ++i) if (g.sn[i].x == 0u) end = std::max<size_t>(end, (size_t) g.first(i, which) + g.count[i]);
+    if (end > h->capPool) return fail(PPG_ERR_CUDA, "SD-tree leaf points past the quadtree pool");
+    g.children.resize(end); g.sums.resize(end);
+    if (which) {
+        CK(cudaMemcpy(g.children.data(), h->dBchildren.p, sizeof(uint2) * end, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.sums.data(), h->dTrain.p, sizeof(float4) * end, cudaMemcpyDeviceToHost));
+    } else {
+        std::vector<SampNode> pool(end);
+        CK(cudaMemcpy(pool.data(), h->dSamp.p, sizeof(SampNode) * end, cudaMemcpyDeviceToHost));
+        for (size_t k = 0; k < end; ++k) { g.children[k] = pool[k].children; g.sums[k] = pool[k].sums; }
+    }
+    return PPG_OK;
+}
+
+extern "C" int ppg_export_sdtree(ppg_integrator *h, int which, size_t node_capacity, size_t *n_nodes_out, uint32_t *node_children, uint64_t *tree_first,
+                                 uint32_t *tree_count, int32_t *tree_depth, float *tree_sum, float *tree_weight, float *adam,
+                                 size_t pool_capacity, size_t *n_pool_out, float *sums, uint16_t *children, float *aabb_min_max) {
+  return guarded("ppg_export_sdtree", [&]() -> int {
+    if (!h || !n_nodes_out || !n_pool_out || (which != 0 && which != 1)) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_export_sdtree: null argument or `which` not 0 / 1");
+    TreeGather g; int rc = gather_tree(h, which, g); if (rc) return rc;
+    size_t total = 0;
+    for (uint32_t i = 0; i < g.n; ++i) if (g.sn[i].x == 0u) total += g.count[i];
+    *n_nodes_out = g.n; *n_pool_out = total;
+    if (g.n > node_capacity || total > pool_capacity)
+        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_export_sdtree: output arrays too small (*n_nodes_out and *n_pool_out hold the sizes needed)");
+    uint64_t off = 0;
+    for (uint32_t i = 0; i < g.n; ++i) {          // inner nodes carry no tree and no optimiser state (STree::subdivide, GP:876-895)
+        const bool leaf = g.sn[i].x == 0u;
+        if (node_children) { node_children[2 * i] = g.sn[i].x; node_children[2 * i + 1] = g.sn[i].y; }
+        if (tree_first) tree_first[i] = off;
+        if (tree_count) tree_count[i] = leaf ? g.count[i] : 0u;
+        if (tree_depth) tree_depth[i] = leaf ? g.depth[i] : 0;
+        if (tree_sum) tree_sum[i] = leaf ? g.sum[i] : 0.f;
+        if (tree_weight) tree_weight[i] = leaf ? g.weight[i] : 0.f;
+        if (adam) {
+            for (int j = 0; j < 6; ++j) adam[6 * (size_t) i + j] = leaf ? g.adam[6 * (size_t) i + j] : 0.f;
+            if (leaf) adam[6 * (size_t) i + 3] = g.la[i].z;           // theta as the bounce kernel reads it
+        }
+        if (!leaf) continue;
+        const uint32_t base = g.first(i, which);
+        for (uint32_t k = 0; k < g.count[i]; ++k) {
+            const float4 s = g.sums[base + k]; const uint2 c = g.children[base + k];
+            if (sums) { float *o = sums + 4 * (off + k); o[0] = s.x; o[1] = s.y; o[2] = s.z; o[3] = s.w; }
+            if (children) { uint16_t *o = children + 4 * (off + k); o[0] = (uint16_t) (c.x & 0xffff); o[1] = (uint16_t) (c.x >> 16); o[2] = (uint16_t) (c.y & 0xffff); o[3] = (uint16_t) (c.y >> 16); }
+        }
+        off += g.count[i];
+    }
+    if (aabb_min_max) {                           // the cubified box of the S-tree (STree::STree, GP:850-860; pack_scene)
+        const float m = std::max(std::max(h->aabbMax[0] - h->aabbMin[0], h->aabbMax[1] - h->aabbMin[1]), h->aabbMax[2] - h->aabbMin[2]);
+        for (int a = 0; a < 3; ++a) { aabb_min_max[a] = h->aabbMin[a]; aabb_min_max[3 + a] = h->aabbMin[a] + m; }
+    }
+    return PPG_OK;
+  });
+}
+
 // dumpSDTree wire format (GP:1191-1208, 699-711, 945-951): 16 floats camera matrix, then for every leaf with
 // sampling weight > 0, in forEachLeaf order (child 0 before child 1): pos, size, mean, u64 weight, u64 nNodes,
 // nNodes x 4 x (f32 sum, u16 child)
@@ -1187,17 +1264,8 @@ static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path);
 extern "C" int ppg_dump_sdtree(ppg_integrator *h, const char *path) { return guarded("ppg_dump_sdtree", [&] { return ppg_dump_sdtree_impl(h, path); }); }
 static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path) {
     if (!h || !path) return fail(PPG_ERR_INVALID_ARGUMENT, "null argument");
-    if (!h->haveScene || h->capNodes == 0) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
-    CK(cudaSetDevice(h->device));
-    const uint32_t n = h->hNodes;
-    std::vector<uint2> sn(n); std::vector<float4> la(n); std::vector<float> ssum(n), sw(n); std::vector<uint32_t> scnt(n);
-    CK(cudaMemcpy(sn.data(), h->dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(la.data(), h->dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(ssum.data(), h->dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(sw.data(), h->dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(scnt.data(), h->dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    std::vector<SampNode> pool(std::max<size_t>(h->hTotalBuild, 1));
-    CK(cudaMemcpy(pool.data(), h->dSamp.p, sizeof(SampNode) * pool.size(), cudaMemcpyDeviceToHost));
+    TreeGather g; int rc = gather_tree(h, 0, g); if (rc) return rc;
+    const std::vector<uint2> &sn = g.sn; const std::vector<float> &ssum = g.sum, &sw = g.weight; const std::vector<uint32_t> &scnt = g.count;
     FILE *f = fopen(path, "wb");
     if (!f) return fail(PPG_ERR_IO, std::string("cannot open ") + path);
     float cm[16];
@@ -1217,12 +1285,11 @@ static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path) {
             fwrite(e.p, 4, 3, f); fwrite(e.s, 4, 3, f); fwrite(&mean, 4, 1, f);
             const uint64_t w64 = (uint64_t) sw[e.n], nn = scnt[e.n];
             fwrite(&w64, 8, 1, f); fwrite(&nn, 8, 1, f);
-            uint32_t base; memcpy(&base, &la[e.n].x, 4);
-            if ((size_t) base + scnt[e.n] > pool.size()) { fclose(f); return fail(PPG_ERR_IO, "SD-tree is being rebuilt (render cancelled between reset and build): nothing consistent to dump"); }
+            const uint32_t base = g.first(e.n, 0);
             for (uint32_t k = 0; k < scnt[e.n]; ++k) {
-                const SampNode &q = pool[base + k];
-                const float s4[4] = {q.sums.x, q.sums.y, q.sums.z, q.sums.w};
-                const uint16_t c4[4] = {(uint16_t) (q.children.x & 0xffff), (uint16_t) (q.children.x >> 16), (uint16_t) (q.children.y & 0xffff), (uint16_t) (q.children.y >> 16)};
+                const float4 &s = g.sums[base + k]; const uint2 &c = g.children[base + k];
+                const float s4[4] = {s.x, s.y, s.z, s.w};
+                const uint16_t c4[4] = {(uint16_t) (c.x & 0xffff), (uint16_t) (c.x >> 16), (uint16_t) (c.y & 0xffff), (uint16_t) (c.y >> 16)};
                 for (int j = 0; j < 4; ++j) { fwrite(&s4[j], 4, 1, f); fwrite(&c4[j], 2, 1, f); }
             }
         } else {

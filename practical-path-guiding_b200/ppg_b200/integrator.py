@@ -150,6 +150,23 @@ class GuidedPathTracer:
     def dump_sdtree(self, path: str):
         _check(self.lib, self.lib.ppg_dump_sdtree(self._h, path.encode()))
 
+    def export_sdtree(self, which: int = 0):
+        """The SD-tree as flat arrays (ppg_export_sdtree), after render() or from inside the film callback; which: 0 = sampling trees,
+        1 = building trees.  Returns a dict: s_children (N, 2), tree_first / tree_count / tree_depth /
+        tree_sum / tree_weight (N,), adam (N, 6), sums (M, 4), children (M, 4) uint16, aabb (2, 3)."""
+        nn, nq = C.c_size_t(), C.c_size_t()
+        rc = self.lib.ppg_export_sdtree(self._h, which, 0, C.byref(nn), None, None, None, None, None, None, None, 0, C.byref(nq), None, None, None)
+        _check(self.lib, rc, allow=(-1,) if nn.value or nq.value else ())      # -1 with the sizes filled in: the arrays were too small
+        N, M = nn.value, nq.value
+        e = dict(s_children=np.zeros((N, 2), np.uint32), tree_first=np.zeros(N, np.uint64), tree_count=np.zeros(N, np.uint32), tree_depth=np.zeros(N, np.int32),
+                 tree_sum=np.zeros(N, np.float32), tree_weight=np.zeros(N, np.float32), adam=np.zeros((N, 6), np.float32), sums=np.zeros((M, 4), np.float32),
+                 children=np.zeros((M, 4), np.uint16), aabb=np.zeros((2, 3), np.float32))
+        P = lambda k, t: e[k].ctypes.data_as(C.POINTER(t))
+        _check(self.lib, self.lib.ppg_export_sdtree(self._h, which, N, C.byref(nn), P("s_children", C.c_uint32), P("tree_first", C.c_uint64), P("tree_count", C.c_uint32),
+                                                    P("tree_depth", C.c_int32), P("tree_sum", C.c_float), P("tree_weight", C.c_float), P("adam", C.c_float),
+                                                    M, C.byref(nq), P("sums", C.c_float), P("children", C.c_uint16), P("aabb", C.c_float)))
+        return e
+
     def op_emitter_sample_direct(self, ref, ref_n, sample, max_interactions=-1):
         """Scene::sampleAttenuatedEmitterDirect at the points `ref` of this handle's scene (ppg_op_emitter_sample_direct): (d, value, pdf, dist)."""
         f = C.POINTER(C.c_float)

@@ -55,6 +55,8 @@ def _declare(lib):
     lib.ppgo_tree_fraction.argtypes = [H, C.c_size_t, u32p, f32p]
     lib.ppgo_tree_counts.argtypes = [H, u64p]
     lib.ppgo_tree_export.argtypes = [H, C.c_int, u32p, i32p, u8p, u64p, u32p, f32p, f32p, i32p, f32p, u16p, f32p, f32p]
+    if hasattr(lib, "ppgo_tree_import"):                # as ppgo_tree_sample_canonical
+        lib.ppgo_tree_import.argtypes = [H, C.c_size_t, u32p, u64p, u32p, f32p, f32p, i32p, f32p, u16p, C.c_size_t, f32p, C.c_int, C.c_int]
     return lib
 
 
@@ -301,6 +303,16 @@ class Oracle:
                                   P(e["children"], C.c_uint16), P(e["adam"], C.c_float), P(e["aabb"], C.c_float))
         e["n_leaves"] = int(cnt[1])
         return e
+
+    def import_tree(self, e, iter=0, passes_rendered=0):
+        """Replace the tree by a sampling-side export `e` (this class's export(0) or GuidedPathTracer.export_sdtree(0)); with a scene, the next
+        step_passes continues after `passes_rendered` passes of iteration `iter`.  Returns the status (-6 on the verbatim reference backend)."""
+        C_ = lambda k, t: np.ascontiguousarray(e[k], t)
+        a = dict(sc=C_("s_children", np.uint32), tf=C_("tree_first", np.uint64), tc=C_("tree_count", np.uint32), ts=C_("tree_sum", np.float32),
+                 tw=C_("tree_weight", np.float32), td=C_("tree_depth", np.int32), s=C_("sums", np.float32), c=C_("children", np.uint16), ad=C_("adam", np.float32))
+        P = lambda k, t: a[k].ctypes.data_as(C.POINTER(t))
+        return self.lib.ppgo_tree_import(self.h, len(a["sc"]), P("sc", C.c_uint32), P("tf", C.c_uint64), P("tc", C.c_uint32), P("ts", C.c_float), P("tw", C.c_float),
+                                         P("td", C.c_int32), P("s", C.c_float), P("c", C.c_uint16), len(a["s"]), P("ad", C.c_float), iter, passes_rendered)
 
 
 def make_bsdf(type=0, flags=0, reflectance=(0.5, 0.5, 0.5), transmittance=(1, 1, 1), eta=(1.5, 1.5, 1.5), k=(0, 0, 0), alpha=0.1, distribution=1):

@@ -221,3 +221,60 @@ def test_restated_commit_equals_the_reference_vertex_commit(sfilter, dfilter, lo
             o.build()
     refgold.check(f"sdtree/commit_equals_the_reference_vertex_commit/{sfilter}{dfilter}{loss}", mine, (lambda: ref) if ref else None)
     assert trees["restated on port trees"].commit(pos, d, thr, bv, radiance, wo, bp, dp, weight, delta, rnd, verbatim=True) == -6      # no reference code in the restated build
+
+
+def _export_keys(e):
+    return {k: e[k] for k in ("s_children", "s_axis", "s_is_leaf", "tree_first", "tree_count", "tree_depth", "tree_sum", "tree_weight", "sums", "children", "adam", "aabb")}
+
+
+def test_tree_import_round_trips_the_export():
+    """ppgo_tree_import is the inverse of the sampling-side export: a trained tree (box filters, KL loss: leaves at many depths, nonzero Adam
+    state) exported, imported into a fresh handle and exported again gives the same arrays bit for bit, axes included (they follow from the
+    depth).  Arrays that are not a tree are refused, and the verbatim reference backend has no import."""
+    o, _ = _run("port", 2, 1, 1, iters=3, n=3000)
+    e = o.export(0)
+    assert e["n_leaves"] > 8 and np.abs(e["adam"][:, 3]).max() > 0
+    fresh = O.Oracle(O.default_params(), aabb=AABB)
+    assert fresh.import_tree(e) == 0
+    got, want = _export_keys(fresh.export(0)), _export_keys(e)
+    for k in want:
+        assert np.array_equal(got[k].view(np.uint8), want[k].view(np.uint8)), k
+    bad = dict(e); bad["s_children"] = e["s_children"].copy(); bad["s_children"][0] = [1, 1]      # a node reached twice
+    assert fresh.import_tree(bad) == -1
+    bad = dict(e); bad["tree_count"] = e["tree_count"].copy(); bad["tree_count"][np.argmax(e["s_is_leaf"])] = len(e["sums"]) + 1
+    assert fresh.import_tree(bad) == -1
+    if O.have_ref():
+        ref = O.Oracle(O.default_params(), aabb=AABB, kind="ref")
+        if hasattr(ref.lib, "ppgo_tree_import"):
+            assert ref.import_tree(e) == -6
+
+
+@pytest.mark.parametrize("loss,final", [("none", False), ("kl", True)])
+def test_imported_tree_renders_the_next_pass_bit_for_bit(loss, final):
+    """An oracle trained on CBOX 64^2 for two iterations (1 + 2 passes), refined and reset for the third, against a fresh oracle that gets only
+    its tree (ppgo_tree_import) and its pass count, then resets its building trees the same way: the next pass follows the same paths, so the
+    moment images are equal bit for bit, and (single-threaded, same record order) so are the building trees.  loss=kl on the final pass: every
+    vertex uses its leaf's learned fraction."""
+    from common import load_cbox
+    sc = load_cbox(64)
+    props = dict(sc.integrator, budget="28", rrDepth="5", nee="kickstart", bsdfSamplingFraction="0.3", bsdfSamplingFractionLoss=loss)
+    p = O.params_from_xml(props)
+    a = O.Oracle(p, sc, nthreads=1)
+    a.step_reset(0); a.step_passes(1); a.step_build()
+    a.step_reset(1); a.step_passes(2); a.step_build()
+    a.step_reset(2)                                   # refine + reset of iteration 2
+    e = a.export(0)
+    if loss == "kl":
+        assert np.abs(e["adam"][e["s_is_leaf"] == 1, 3]).max() > 0.01       # the fractions have moved
+    b = O.Oracle(p, sc, nthreads=1)
+    assert b.import_tree(e, iter=2, passes_rendered=3) == 0
+    b.reset(20, p.d_tree_threshold)
+    a.step_passes(1, is_final=final); b.step_passes(1, is_final=final)
+    for x, y in zip(a.moment_images(), b.moment_images()):
+        assert x[..., 3].sum() == 64 * 64 * 4
+        assert np.array_equal(x, y)
+    ea, eb = a.export(1), b.export(1)
+    for k in ("s_children", "tree_count", "tree_depth", "tree_weight", "sums", "children", "adam"):
+        assert np.array_equal(ea[k], eb[k]), k
+    if not final:
+        assert ea["tree_weight"].sum() > 1000
