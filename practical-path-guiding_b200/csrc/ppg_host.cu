@@ -221,7 +221,7 @@ struct ppg_integrator {
     ppg_clock_fn clockFn = nullptr; void *clockUser = nullptr; ppg_film_fn filmFn = nullptr; void *filmUser = nullptr;
     float clock_s() const { return clockFn ? (float) clockFn(clockUser) : (float) std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - startTime).count() / 1000; }
     unsigned long long adamProgress[2] = {0, 0};          // [sum steps * |df| * 2^20, sum steps] of the last Adam replay
-    uint64_t lastRecorded = 0;                             // guiding records of the last performRenderPasses (this rank): bounds the growth of the S-tree
+    uint64_t lastRecorded = 0;                             // guiding records of the last performRenderPasses (all ranks): bounds the growth of the S-tree
 
     // scene
     bool haveScene = false;
@@ -590,8 +590,8 @@ static int reset_sd_tree(ppg_integrator *h) {
     }
     if (!memCapped) {
         // capacity: the refinement creates at most 2 nodes per threshold worth of recorded weight.  The total weight of the iteration is at most
-        // its number of guiding records (weights <= 1); with several ranks the reduced weights hold about world x this rank's records.
-        const double totalW = 1.25 * (double) h->lastRecorded * h->world + 4096;
+        // its number of guiding records (weights <= 1), summed over the ranks whose weights are reduced.
+        const double totalW = 1.25 * (double) h->lastRecorded + 4096;
         const double est = refine_capacity(h->hNodes, totalW, threshold);
         int rc = ensure_tree_capacity(h, (uint32_t) std::min<double>(est, 4.0e9), h->capPool);
         if (rc) return rc;
@@ -876,11 +876,11 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
                                                               lossMode == PPG_LOSS_KL ? 1.0f : 2.0f); h->launches++;
         h->toc();
         if (multi) {
-            // replicas replayed their own records from the common state: merge them (step counts and batch accumulators add up relative to
-            // the common start, moments and the variable are averaged) so that all ranks continue identically
+            // replicas replayed their own records from the common state: merge them (steps and moves of the variable add up, moments are
+            // weighted by the steps, batch accumulators add up relative to the common start) so that all ranks continue identically
             adam_pack_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, nullptr, 1); h->launches++;
             int rc = allreduce_sum(h, tail, 6 * (size_t) h->hNodes); if (rc) return rc;
-            adam_merge_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, 1.0f / (float) h->world, (float) (h->world - 1)); h->launches++;
+            adam_merge_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, (float) (h->world - 1)); h->launches++;
         }
         // movement of the fractions in this replay (identical on all ranks after the merge): steers the size of the next sub-batch
         CK(cudaMemsetAsync(h->dCounters.p + 6, 0, 16, h->stream));
@@ -965,7 +965,8 @@ static int perform_render_passes(ppg_integrator *h, float &variance, int numPass
         else std::rotate(h->images.begin(), h->images.begin() + 1, h->images.end());
         CK(cudaMemcpyAsync(h->images.back()->p, h->dImage.p, sizeof(float4) * npx, cudaMemcpyDeviceToDevice, h->stream));
     }
-    // variance, GP:1298-1319: the numerator is reduced on the device (double), summed over ranks as a float, and read back together with the counters
+    // variance, GP:1298-1319: the numerator is reduced on the device (double), summed over ranks as a float together with the guiding records
+    // (the next refine's capacity), and read back with the counters
     const int N = local * h->prm.spp_per_pass;
     CK(cudaMemsetAsync(h->dVar.p, 0, 8, h->stream));
     if (h->nLocalPixels)
@@ -973,15 +974,16 @@ static int perform_render_passes(ppg_integrator *h, float &variance, int numPass
             h->dImage.p, h->dSqImage.p, h->dPixelMap.p, h->nLocalPixels, h->W, (float) N, h->dVar.p);
     h->launches++;
     float *slot = h->dTrain.p + h->dTrain.n - 16;
-    double_to_float_kernel<<<1, 1, 0, h->stream>>>(h->dVar.p, slot); h->launches++;
-    if (h->multi()) { int rc = allreduce_sum(h, slot, 1); if (rc) return rc; }
-    float numF = 0; unsigned long long cnt[8];
-    CK(cudaMemcpyAsync(&numF, slot, 4, cudaMemcpyDeviceToHost, h->stream));
+    iteration_scalars_kernel<<<1, 1, 0, h->stream>>>(h->dVar.p, h->dCounters.p, slot); h->launches++;
+    if (h->multi()) { int rc = allreduce_sum(h, slot, 2); if (rc) return rc; }
+    float reduced[2] = {0, 0}; unsigned long long cnt[8];
+    CK(cudaMemcpyAsync(reduced, slot, 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(cnt, h->dCounters.p, 64, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaEventRecord(h->evB, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     float ms = 0; cudaEventElapsedTime(&ms, h->evA, h->evB); h->deviceMs += ms;
     h->resolve_timers();
+    const float numF = reduced[0];
     variance = (float) ((double) numF / ((double) h->W * h->H * (N - 1)));
     if (h->prm.sample_combination == PPG_COMB_INVERSEVAR) { h->variances.push_back(variance); if (h->variances.size() > 4) h->variances.erase(h->variances.begin()); }
     st.seconds += elapsed_s(t0); st.passes += local; st.variance = variance; st.total_passes = h->passesRendered;
@@ -989,7 +991,8 @@ static int perform_render_passes(ppg_integrator *h, float &variance, int numPass
     if (cnt[1]) st.s_tree_depth_avg = (double) cnt[2] / (double) cnt[1];
     h->stats.total_vertices += cnt[0]; h->stats.total_paths += (uint64_t) local * perPass;
     h->stats.truncated_paths += cnt[3]; h->stats.dropped_records += cnt[4]; h->stats.invalid_rays += cnt[5];
-    h->lastRecorded = cnt[1];
+    // every rank sizes the next refine from the same count: the records of all ranks (a rank that owns few pixels would size too small a tree)
+    h->lastRecorded = h->multi() ? (uint64_t) reduced[1] : cnt[1] * (uint64_t) h->world;
     static const int trace = env_int("PPG_TRACE", 0);
     if (trace)    // cumulative kernel times after every iteration's passes (stderr): where a render's time goes, iteration by iteration
         fprintf(stderr, "[ppg trace] iter %d final %d passes %d sub_batches %llu vertices %llu entered at %.1f ms wall %.1f ms | cumulative ms: bounce %.1f commit %.1f adam %.1f other %.1f film %.1f launches %llu\n",

@@ -537,25 +537,31 @@ __global__ void __launch_bounds__(128) adam_seq_kernel(const __grid_constant__ M
         }
     }
 }
-// N > 1 ranks: every rank replays its own records from the common state; the replicas are then merged.  The exchange buffer holds the SUM over
-// ranks of [iter - iterBefore | m1 | m2 | variable | batchAcc | batchGrad] (6 arrays of nNodes floats).  Step counts add up, moments and the
-// variable are averaged, and the batch accumulators add up RELATIVE to the common start (each rank's value contains the carried-over part once).
+// N > 1 ranks: every rank replays its own records from the common state; the replicas are then merged as if one optimiser had taken all their
+// steps.  The exchange buffer holds the SUM over ranks of [ds | ds * m1 | ds * m2 | theta - thetaBefore | batchAcc | batchGrad] (6 arrays of
+// nNodes floats; ds = iter - iterBefore, this replica's steps).  Step counts add up; the variable moves by the sum of the replicas' moves, so a
+// replica that took no step contributes nothing (averaging would move it 1/world as far as the reference's single optimiser); the moments are
+// the step-weighted mean of the replicas' (unchanged when no replica stepped); the batch accumulators add up RELATIVE to the common start (each
+// rank's value contains the carried-over part once).
 __global__ void adam_pack_kernel(const __grid_constant__ MaintParams M, float *out6, float *before3, const float *unused, int stage) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {
         const float *st = M.adam + 6 * (size_t) n;
         if (stage == 0) { before3[n] = st[0]; before3[(size_t) nNodes + n] = st[4]; before3[2 * (size_t) nNodes + n] = st[5]; before3[3 * (size_t) nNodes + n] = st[3]; continue; }   // before the replay
-        out6[n] = st[0] - before3[n];
-        out6[(size_t) nNodes + n] = st[1]; out6[2 * (size_t) nNodes + n] = st[2]; out6[3 * (size_t) nNodes + n] = st[3];
+        const float ds = st[0] - before3[n];
+        out6[n] = ds;
+        out6[(size_t) nNodes + n] = ds * st[1]; out6[2 * (size_t) nNodes + n] = ds * st[2]; out6[3 * (size_t) nNodes + n] = st[3] - before3[3 * (size_t) nNodes + n];
         out6[4 * (size_t) nNodes + n] = st[4]; out6[5 * (size_t) nNodes + n] = st[5];
     }
 }
-__global__ void adam_merge_kernel(const __grid_constant__ MaintParams M, const float *sum6, const float *before3, float invWorld, float worldMinus1) {
+__global__ void adam_merge_kernel(const __grid_constant__ MaintParams M, const float *sum6, const float *before3, float worldMinus1) {
     const uint32_t nNodes = *M.nNodes;
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < nNodes; n += gridDim.x * blockDim.x) {
         float *st = M.adam + 6 * (size_t) n;
-        st[0] = before3[n] + sum6[n];
-        st[1] = sum6[(size_t) nNodes + n] * invWorld; st[2] = sum6[2 * (size_t) nNodes + n] * invWorld; st[3] = sum6[3 * (size_t) nNodes + n] * invWorld;
+        const float ds = sum6[n];
+        st[0] = before3[n] + ds;
+        if (ds > 0.f) { st[1] = sum6[(size_t) nNodes + n] / ds; st[2] = sum6[2 * (size_t) nNodes + n] / ds; }
+        st[3] = fminf(fmaxf(before3[3 * (size_t) nNodes + n] + sum6[3 * (size_t) nNodes + n], -20.0f), 20.0f);
         const float acc = sum6[4 * (size_t) nNodes + n] - worldMinus1 * before3[(size_t) nNodes + n];
         const float grad = sum6[5 * (size_t) nNodes + n] - worldMinus1 * before3[2 * (size_t) nNodes + n];
         st[4] = acc > 0.f ? acc : 0.f; st[5] = acc > 0.f ? grad : 0.f;
@@ -627,6 +633,7 @@ __global__ void adam_progress_kernel(const __grid_constant__ MaintParams M, cons
     for (int off = 16; off; off >>= 1) { moved += __shfl_xor_sync(0xffffffffu, moved, off); steps += __shfl_xor_sync(0xffffffffu, steps, off); }
     if ((threadIdx.x & 31) == 0 && steps) { atomicAdd(&out2[0], moved); atomicAdd(&out2[1], steps); }
 }
-__global__ void double_to_float_kernel(const double *in, float *out) { *out = (float) *in; }
+// the per-iteration scalars the ranks sum (perform_render_passes): [variance numerator, guiding records]
+__global__ void iteration_scalars_kernel(const double *variance, const unsigned long long *counters, float *out) { out[0] = (float) *variance; out[1] = (float) counters[1]; }
 
 }  // namespace ppg

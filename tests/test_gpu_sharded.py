@@ -57,6 +57,6 @@ def test_library_nccl_communicator_matches_single_rank():
     img, st = g.render()
     w = [i["weight_avg"] * i["s_tree_leaves"] for i in st["iterations"]]
     # (16 - 48 leaves and the sampling fractions in fast transit: the recorded count of the learning iterations of this small configuration
-    # varies by +-10 % from run to run on ONE rank already; the ranks merge their optimiser replicas by averaging)
+    # varies by +-10 % from run to run on ONE rank already)
     assert r0["weights"][0] == w[0] and np.allclose(r0["weights"], w, rtol=0.15)
     assert abs(r0["img"].mean() - img.mean()) <= 0.02 * img.mean()
