@@ -204,6 +204,219 @@ extern "C" int ppg_scene_file_load(const char *path, ppg_scene_desc *d, ppg_scen
 }
 extern "C" void ppg_scene_file_free(ppg_scene_file *file) { delete file; }
 
+// ------------------------------------------------------------------ SD-tree storage and its launch sequences
+static float bits_f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
+static uint32_t f_bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+static std::vector<SampNode> to_pool(const float *sums, const uint16_t *children, size_t n) {
+    std::vector<SampNode> pool(n);
+    for (size_t i = 0; i < n; ++i) {
+        pool[i].sums = make_float4(sums[4 * i], sums[4 * i + 1], sums[4 * i + 2], sums[4 * i + 3]);
+        pool[i].children = make_uint2((uint32_t) children[4 * i] | ((uint32_t) children[4 * i + 1] << 16), (uint32_t) children[4 * i + 2] | ((uint32_t) children[4 * i + 3] << 16));
+        pool[i].pad = make_uint2(0u, 0u);
+    }
+    return pool;
+}
+
+// An SD-tree on the host: the S-tree and, per node, either the sampling trees (which == 0: the trees the passes guide with) or the
+// building trees (which == 1: the trees the passes record into).  Between the reset and the build of an iteration (the film callback) the sampling
+// trees still sit where the previous build put them, past the new building total: the copy of the quadtree pool is sized from the leaves (or `minPool`).
+struct TreeGather {
+    uint32_t n = 0;
+    std::vector<uint2> sn; std::vector<float4> la; std::vector<float> sum, weight, adam; std::vector<int> depth; std::vector<uint32_t> count;
+    std::vector<uint2> children; std::vector<float4> sums;      // the quadtree pool from offset 0 (building: bchildren / bsums; sampling: dSamp)
+    uint32_t first(uint32_t i, int which) const { uint32_t u; memcpy(&u, which ? &la[i].y : &la[i].x, 4); return u; }
+};
+
+// The SD-tree on the device and its launch sequences, shared by the render and the ppg_op_* entry points.  Launch members return their launch count.
+struct TreeStore {
+    cudaStream_t stream = nullptr; int numSMs = 132, commitGrid = 0;
+    uint32_t capNodes = 0; size_t capPool = 0;
+    DevBuf<uint2> dSnodes; DevBuf<float4> dLeafA; DevBuf<float> dBweight, dSampSum, dSampWeight, dAdam, dAdamBefore /* 4 x capNodes: iter, batchAcc, batchGrad, theta before a replay */;
+    DevBuf<uint32_t> dAdamCount, dAdamCursor, dAdamOffset; DevBuf<float4> dAdamRecA, dAdamSortA; DevBuf<float2> dAdamRecB, dAdamSortB; size_t adamCap = 0;
+    DevBuf<int> dSampDepth, dBuildDepth; DevBuf<uint32_t> dSampCount, dBuildCount, dBuildBase, dScalars /* [0]=nNodes [1]=totalBuild */;
+    DevBuf<uint32_t> dStable; DevBuf<TreeStats> dTreeStats;
+    DevBuf<SampNode> dSamp; DevBuf<uint2> dBchildren; DevBuf<float> dTrain /* bsums | packed tail */;
+    uint32_t hNodes = 1; uint32_t hTotalBuild = 1;
+    static constexpr size_t kTableEntries = (size_t) 1 << (3 * PPG_STREE_TABLE_BITS);
+
+    // the whole buffer zeroed, then its first n elements copied from the host (host may be null: zeros)
+    template <class T> cudaError_t put(DevBuf<T> &b, const void *host = nullptr, size_t n = 0) {
+        cudaError_t e = cudaMemsetAsync(b.p, 0, b.n * sizeof(T), stream); if (e != cudaSuccess) return e;
+        return (host && n) ? cudaMemcpyAsync(b.p, host, n * sizeof(T), cudaMemcpyHostToDevice, stream) : cudaSuccess;
+    }
+
+    // room for `nodes` S-tree nodes and `pool` quadtree nodes: grown by doubling (the render), or to exactly that size
+    int reserve(uint32_t nodes, size_t pool, bool exact = false) {
+        CK(dScalars.alloc(8)); CK(dTreeStats.alloc(1));
+        if (nodes > capNodes) {
+            const uint32_t cap = exact ? nodes : std::max<uint32_t>(nodes, std::max<uint32_t>(2 * capNodes, 1u << 16));
+            CK(dSnodes.grow(cap, stream)); CK(dLeafA.grow(cap, stream)); CK(dBweight.grow(cap, stream));
+            CK(dSampSum.grow(cap, stream)); CK(dSampWeight.grow(cap, stream)); CK(dAdam.grow(6 * (size_t) cap, stream));
+            CK(dAdamBefore.grow(4 * (size_t) cap, stream)); CK(dSampDepth.grow(cap, stream));
+            {   // record-bucket bookkeeping must stay zero between commit launches: reallocate zeroed
+                dAdamCount.release(); dAdamCursor.release(); dAdamOffset.release();
+                CK(dAdamCount.alloc(cap)); CK(dAdamCursor.alloc(cap)); CK(dAdamOffset.alloc(cap));
+                CK(cudaMemsetAsync(dAdamCount.p, 0, 4 * (size_t) cap, stream)); CK(cudaMemsetAsync(dAdamCursor.p, 0, 4 * (size_t) cap, stream));
+            }
+            CK(dBuildDepth.grow(cap, stream)); CK(dSampCount.grow(cap, stream)); CK(dBuildCount.grow(cap, stream));
+            CK(dBuildBase.grow(cap, stream));
+            capNodes = cap;
+        }
+        if (pool > capPool) {
+            const size_t cap = exact ? pool : std::max<size_t>(pool, std::max<size_t>(2 * capPool, (size_t) 1 << 20));
+            CK(dSamp.grow(cap, stream)); CK(dBchildren.grow(cap, stream));
+            capPool = cap;
+        }
+        // bsums (4 floats per pool node) followed by the packed exchange tail (building weights, or 6 Adam arrays; + scalars)
+        CK(dTrain.grow(4 * capPool + 6 * (size_t) capNodes + 64, stream));
+        return PPG_OK;
+    }
+
+    MaintParams maint() const {
+        MaintParams M;
+        M.snodes = dSnodes.p; M.leafA = dLeafA.p; M.bweight = dBweight.p; M.sampSum = dSampSum.p; M.sampWeight = dSampWeight.p;
+        M.sampDepth = dSampDepth.p; M.sampCount = dSampCount.p; M.adam = dAdam.p; M.buildCount = dBuildCount.p; M.buildDepth = dBuildDepth.p;
+        M.nNodes = dScalars.p; M.capNodes = capNodes; M.samp = dSamp.p; M.bchildren = dBchildren.p; M.bsums = reinterpret_cast<float4 *>(dTrain.p);
+        return M;
+    }
+    TreeView view(const float *aabbMin, const float *extent) const {
+        TreeView T;
+        T.snodes = dSnodes.p; T.stable = stree_table_usable(hNodes) ? dStable.p : nullptr; T.leafA = dLeafA.p; T.samp = dSamp.p; T.bchildren = dBchildren.p;
+        T.bsums = reinterpret_cast<float4 *>(dTrain.p); T.bweight = dBweight.p;
+        T.aabbMin = make_float3(aabbMin[0], aabbMin[1], aabbMin[2]); T.extent = make_float3(extent[0], extent[1], extent[2]);
+        return T;
+    }
+
+    // new STree (GP:1519): one leaf whose sampling tree is a single empty quadtree node
+    int init() {
+        // buffers persist across renders (cudaMalloc/cudaFree are synchronous and slow): only their contents are reset
+        int rc = reserve(std::max<uint32_t>(capNodes, 1u << 16), std::max<size_t>(capPool, (size_t) 1 << 20));
+        if (rc) return rc;
+        const uint32_t one[2] = {1u, 1u};
+        CK(put(dScalars, one, 2));
+        CK(put(dSnodes)); CK(put(dLeafA)); CK(put(dBweight)); CK(put(dSampSum)); CK(put(dSampWeight));
+        CK(put(dAdam)); CK(put(dAdamCount)); CK(put(dAdamCursor)); CK(put(dSampDepth));
+        CK(cudaMemsetAsync(dSamp.p, 0, sizeof(SampNode), stream));          // one empty quadtree node at pool offset 0
+        CK(cudaMemcpyAsync(dSampCount.p, one, 4, cudaMemcpyHostToDevice, stream));
+        hNodes = 1; hTotalBuild = 1;
+        CK(cudaStreamSynchronize(stream));
+        return PPG_OK;
+    }
+
+    // The flat arrays of the ppg_op_* entry points (null: zeros) on the default stream, in exactly `nodeCap` S-tree and `nPool` quadtree nodes;
+    // first / count / depth / weight and the pool are the sampling trees (which == 0) or the building trees (which == 1)
+    int load(int which, size_t n, uint32_t nodeCap, const uint32_t *nodeChildren, const uint32_t *first, const uint32_t *count, const int32_t *depth,
+             const float *sum, const float *weight, const float *adam, size_t nPool, const float *sums, const uint16_t *children) {
+        int dev = 0;
+        CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev)); CK(dStable.alloc(kTableEntries));
+        int rc = reserve(std::max<uint32_t>(nodeCap, 1), std::max<size_t>(nPool, 1), true); if (rc) return rc;
+        std::vector<float4> la(n);
+        for (size_t i = 0; i < n; ++i) {
+            const float f = bits_f(first ? first[i] : 0u);
+            la[i] = make_float4(f, which ? f : 0.f, adam ? adam[6 * i + 3] : 0.f, 0.f);
+        }
+        CK(put(dSnodes, nodeChildren, n)); CK(put(dLeafA, la.data(), n)); CK(put(dAdam, adam, 6 * n)); CK(put(dSampSum, sum, n));
+        CK(put(dSampWeight, which ? nullptr : weight, n)); CK(put(dSampCount, which ? nullptr : count, n)); CK(put(dSampDepth, which ? nullptr : depth, n));
+        CK(put(dBweight, which ? weight : nullptr, n)); CK(put(dBuildCount, which ? count : nullptr, n)); CK(put(dBuildDepth, which ? depth : nullptr, n));
+        CK(put(dBuildBase, which ? first : nullptr, n));
+        const std::vector<SampNode> pool = which ? std::vector<SampNode>() : to_pool(sums, children, nPool);
+        // the building pool's children keep the ABI's bytes: uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
+        CK(put(dSamp, pool.data(), pool.size())); CK(put(dBchildren, which ? children : nullptr, nPool)); CK(put(dTrain, which ? sums : nullptr, 4 * nPool));
+        const uint32_t sc[8] = {(uint32_t) n, 0, 0, 0, 0, 0, 0, 0};
+        CK(put(dScalars, sc, 8));
+        hNodes = (uint32_t) n; hTotalBuild = 0;
+        return PPG_OK;
+    }
+
+    // STree::refine at `threshold`; a refine that runs out of node capacity raises the flag sync_counts reports
+    int refine(float threshold) { stree_refine_kernel<<<1, 1024, 0, stream>>>(maint(), threshold, dScalars.p + 5); return 1; }
+    // DTree::reset of every leaf, first half: node count of every new building tree, and their offsets in the pool
+    int reset_count(int maxDepth, float threshold) {
+        dtree_reset_kernel<false><<<numSMs * 4, 128, 0, stream>>>(maint(), nullptr, maxDepth, threshold);
+        exclusive_scan_kernel<<<1, 1024, 0, stream>>>(dBuildCount.p, dBuildBase.p, dScalars.p, dScalars.p + 1);
+        return 2;
+    }
+    // between the halves: read back the S-tree node count and the building pool total (waits for the stream), and make room for them and the table
+    int sync_counts(bool exact = false) {
+        uint32_t sc[8];
+        CK(cudaMemcpyAsync(sc, dScalars.p, 32, cudaMemcpyDeviceToHost, stream));
+        CK(cudaStreamSynchronize(stream));
+        if (sc[5]) return fail(PPG_ERR_CUDA, "S-tree refinement ran out of node capacity");
+        hNodes = sc[0]; hTotalBuild = sc[1];
+        CK(dStable.alloc(kTableEntries));
+        return reserve(hNodes, std::max<size_t>(hTotalBuild, 1), exact);
+    }
+    // second half: write the building trees, point every leaf at its own
+    int reset_fill(int maxDepth, float threshold) {
+        const MaintParams M = maint();
+        dtree_reset_kernel<true><<<numSMs * 4, 128, 0, stream>>>(M, dBuildBase.p, maxDepth, threshold);
+        leaf_after_reset_kernel<<<numSMs * 4, 256, 0, stream>>>(M, dBuildBase.p);
+        return 2;
+    }
+    // prefix table of the S-tree (stree_lookup): the first 3 * PPG_STREE_TABLE_BITS levels of every descent become one load.
+    // Past 0xFFFFFF nodes its entries cannot hold the node numbers: view() then hands out no table and the kernels walk from the root.
+    int stree_table() {
+        if (!stree_table_usable(hNodes)) return 0;
+        stree_table_kernel<<<numSMs * 8, 256, 0, stream>>>(dSnodes.p, dStable.p);
+        return 1;
+    }
+    // DTree::build of every leaf; then the distribution statistics (tree_stats_kernel writes the whole record)
+    int build() { dtree_build_kernel<<<numSMs * 4, 128, 0, stream>>>(maint(), dBuildBase.p); return 1; }
+    int tree_stats() { tree_stats_kernel<<<1, 1024, 0, stream>>>(maint(), dTreeStats.p); return 1; }
+    // Vertex::commit into the building trees, gridY rows of blocks (one per slab); sampling-fraction records to dAdamRecA / B, their count to dScalars[3]
+    int commit(CommitParams C, int record, uint32_t nPaths, uint32_t gridY) {
+        if (!commitGrid) {      // resident blocks per SM from the occupancy calculator
+            int occ = 0;
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, commit_kernel<1>, PPG_BLOCK, 0);
+            commitGrid = numSMs * std::max(occ, 1);
+        }
+        C.snodes = dSnodes.p;
+        C.adamRecA = dAdamRecA.p; C.adamRecB = dAdamRecB.p; C.adamTotal = dScalars.p + 3; C.adamCap = (uint32_t) std::min<size_t>(adamCap, 0xFFFFFFFFu);
+        const dim3 g(std::min<int>(commitGrid, (int) ((nPaths + PPG_BLOCK - 1) / PPG_BLOCK)), gridY);
+        if (record == 1) commit_kernel<1><<<g, PPG_BLOCK, 0, stream>>>(C); else commit_kernel<2><<<g, PPG_BLOCK, 0, stream>>>(C);
+        return 1;
+    }
+    // the dScalars[3] records of dAdamRecA / B into per-leaf buckets in dAdamSortA / B (histogram, scan, scatter)
+    int adam_bucket() {
+        adam_hist_kernel<<<numSMs * 4, 256, 0, stream>>>(dAdamRecA.p, dScalars.p + 3, (uint32_t) adamCap, dAdamCount.p);
+        exclusive_scan_kernel<<<1, 1024, 0, stream>>>(dAdamCount.p, dAdamOffset.p, dScalars.p, dScalars.p + 4);
+        adam_scatter_kernel<<<numSMs * 4, 256, 0, stream>>>(dAdamRecA.p, dAdamRecB.p, dScalars.p + 3, (uint32_t) adamCap, dAdamOffset.p,
+                                                            dAdamCursor.p, dAdamSortA.p, dAdamSortB.p);
+        return 3;
+    }
+    int adam_replay(int loss) {
+        adam_seq_kernel<<<numSMs * 16, 128, 0, stream>>>(maint(), dAdamSortA.p, dAdamSortB.p, dAdamOffset.p, dAdamCount.p, dAdamCursor.p,
+                                                         loss == PPG_LOSS_KL ? 1.0f : 2.0f);
+        return 1;
+    }
+
+    int gather(int which, TreeGather &g, size_t minPool = 1) const {
+        if (capNodes == 0) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
+        const uint32_t n = g.n = hNodes;
+        g.sn.resize(n); g.la.resize(n); g.sum.assign(n, 0.f); g.weight.resize(n); g.adam.resize(6 * (size_t) n); g.depth.resize(n); g.count.resize(n);
+        CK(cudaMemcpy(g.sn.data(), dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.la.data(), dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.adam.data(), dAdam.p, 24 * (size_t) n, cudaMemcpyDeviceToHost));
+        if (which == 0) CK(cudaMemcpy(g.sum.data(), dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.weight.data(), which ? dBweight.p : dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.depth.data(), which ? dBuildDepth.p : dSampDepth.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(g.count.data(), which ? dBuildCount.p : dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        size_t end = minPool;
+        for (uint32_t i = 0; i < n; ++i) if (g.sn[i].x == 0u) end = std::max<size_t>(end, (size_t) g.first(i, which) + g.count[i]);
+        if (end > capPool) return fail(PPG_ERR_CUDA, "SD-tree leaf points past the quadtree pool");
+        g.children.resize(end); g.sums.resize(end);
+        if (which) {
+            CK(cudaMemcpy(g.children.data(), dBchildren.p, sizeof(uint2) * end, cudaMemcpyDeviceToHost));
+            CK(cudaMemcpy(g.sums.data(), dTrain.p, sizeof(float4) * end, cudaMemcpyDeviceToHost));
+        } else {
+            std::vector<SampNode> pool(end);
+            CK(cudaMemcpy(pool.data(), dSamp.p, sizeof(SampNode) * end, cudaMemcpyDeviceToHost));
+            for (size_t k = 0; k < end; ++k) { g.children[k] = pool[k].children; g.sums[k] = pool[k].sums; }
+        }
+        return PPG_OK;
+    }
+};
+
 // ------------------------------------------------------------------ the integrator object
 struct ppg_integrator {
     ppg_params prm;
@@ -227,7 +440,7 @@ struct ppg_integrator {
     bool haveScene = false;
     DevBuf<unsigned char> dScene[kSceneArrays]; DevBuf<EnvLight> dEnvLight;     // one buffer per SceneArray (ppg_scene.h)
     SceneView sceneView; Camera cam; uint32_t sceneSmemBytes = 0;
-    float aabbMin[3], aabbMax[3];
+    float aabbMin[3], aabbMax[3], extent[3];
     int W = 0, H = 0;
     DevBuf<uint32_t> dPixelMap, dPixelMapPerm; uint32_t nLocalPixels = 0, minLocalPixels = 0, maxLocalPixels = 0;
 
@@ -235,22 +448,14 @@ struct ppg_integrator {
     DevBuf<float4> dImage, dSqImage, dFilm; DevBuf<float> dRgb; DevBuf<double> dVar;
     std::vector<DevBuf<float4> *> images; std::vector<float> variances;
 
-    // SD-tree
-    uint32_t capNodes = 0; size_t capPool = 0;
-    DevBuf<uint2> dSnodes; DevBuf<float4> dLeafA; DevBuf<float> dBweight, dSampSum, dSampWeight, dAdam, dAdamBefore /* 4 x capNodes: iter, batchAcc, batchGrad, theta before a replay */;
-    DevBuf<uint32_t> dAdamCount, dAdamCursor, dAdamOffset; DevBuf<float4> dAdamRecA, dAdamSortA; DevBuf<float2> dAdamRecB, dAdamSortB; size_t adamCap = 0;
-    DevBuf<int> dSampDepth, dBuildDepth; DevBuf<uint32_t> dSampCount, dBuildCount, dBuildBase, dScalars /* [0]=nNodes [1]=totalBuild */;
-    DevBuf<uint32_t> dStable; DevBuf<TreeStats> dTreeStats;
-    DevBuf<SampNode> dSamp; DevBuf<uint2> dBchildren; DevBuf<float> dTrain /* bsums | packed tail */;
-    uint32_t hNodes = 1; uint32_t hTotalBuild = 1;
-    float extent[3];
+    TreeStore tree;
 
     // wavefront
     size_t pathCapacity = 0; int maxBounces = 0, nSlabs = 0; int recordMode = 0; int stateVecs = 5, slabSets = 1;
     DevBuf<float4> dStateA, dStateB, dSlabs, dLiFinal; DevBuf<uint32_t> dLive, dWork; DevBuf<unsigned long long> dCounters;
     DevBuf<float4> dHits; DevBuf<uint32_t> dTraceWork; int gridTrace = 0; uint32_t traceMinPaths = 0;   // separate nearest-hit pass (ppg_trace.cu), BVH scenes only
     DevBuf<uint32_t> dOrder, dBinCount; bool binMaterials = false;                                        // ... which also bins the paths by the BSDF class they hit
-    int gridBounce = 0, gridCommit = 0;
+    int gridBounce = 0;
 
     // per-kernel-class CUDA-event timing on the launching stream
     struct Timed { cudaEvent_t a, b; int cls; uint32_t launches; };
@@ -313,6 +518,7 @@ extern "C" int ppg_create(const ppg_params *params, int device, ppg_integrator *
     cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, device));
     h->numSMs = prop.multiProcessorCount;
     CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    h->tree.stream = h->stream; h->tree.numSMs = h->numSMs;
     CK(cudaEventCreate(&h->evA)); CK(cudaEventCreate(&h->evB)); CK(cudaEventCreate(&h->evRender0)); CK(cudaEventCreate(&h->evRender1));
     for (auto &e : h->evLive) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     CK(cudaHostAlloc((void **) &h->liveHost, 128 * sizeof(uint32_t), cudaHostAllocDefault));
@@ -506,73 +712,6 @@ static int ppg_set_scene_impl(ppg_integrator *h, const ppg_scene_desc *s) {
     return build_pixel_map(h);
 }
 
-// ------------------------------------------------------------------ SD-tree storage
-static int ensure_tree_capacity(ppg_integrator *h, uint32_t nodes, size_t pool) {
-    if (nodes > h->capNodes) {
-        const uint32_t cap = std::max<uint32_t>(nodes, std::max<uint32_t>(2 * h->capNodes, 1u << 16));
-        CK(h->dSnodes.grow(cap, h->stream)); CK(h->dLeafA.grow(cap, h->stream)); CK(h->dBweight.grow(cap, h->stream));
-        CK(h->dSampSum.grow(cap, h->stream)); CK(h->dSampWeight.grow(cap, h->stream)); CK(h->dAdam.grow(6 * (size_t) cap, h->stream));
-        CK(h->dAdamBefore.grow(4 * (size_t) cap, h->stream)); CK(h->dSampDepth.grow(cap, h->stream));
-        {   // record-bucket bookkeeping must stay zero between commit launches: reallocate zeroed
-            h->dAdamCount.release(); h->dAdamCursor.release(); h->dAdamOffset.release();
-            CK(h->dAdamCount.alloc(cap)); CK(h->dAdamCursor.alloc(cap)); CK(h->dAdamOffset.alloc(cap));
-            CK(cudaMemsetAsync(h->dAdamCount.p, 0, 4 * (size_t) cap, h->stream)); CK(cudaMemsetAsync(h->dAdamCursor.p, 0, 4 * (size_t) cap, h->stream));
-        }
-        CK(h->dBuildDepth.grow(cap, h->stream)); CK(h->dSampCount.grow(cap, h->stream)); CK(h->dBuildCount.grow(cap, h->stream));
-        CK(h->dBuildBase.grow(cap, h->stream));
-        h->capNodes = cap;
-    }
-    if (pool > h->capPool) {
-        const size_t cap = std::max<size_t>(pool, std::max<size_t>(2 * h->capPool, (size_t) 1 << 20));
-        CK(h->dSamp.grow(cap, h->stream)); CK(h->dBchildren.grow(cap, h->stream));
-        h->capPool = cap;
-    }
-    // bsums (4 floats per pool node) followed by the packed exchange tail (building weights, or 6 Adam arrays; + scalars)
-    CK(h->dTrain.grow(4 * h->capPool + 6 * (size_t) h->capNodes + 64, h->stream));
-    return PPG_OK;
-}
-
-static MaintParams maint(ppg_integrator *h) {
-    MaintParams M;
-    M.snodes = h->dSnodes.p; M.leafA = h->dLeafA.p; M.bweight = h->dBweight.p; M.sampSum = h->dSampSum.p; M.sampWeight = h->dSampWeight.p;
-    M.sampDepth = h->dSampDepth.p; M.sampCount = h->dSampCount.p; M.adam = h->dAdam.p; M.buildCount = h->dBuildCount.p; M.buildDepth = h->dBuildDepth.p;
-    M.nNodes = h->dScalars.p; M.capNodes = h->capNodes; M.samp = h->dSamp.p; M.bchildren = h->dBchildren.p; M.bsums = reinterpret_cast<float4 *>(h->dTrain.p);
-    return M;
-}
-
-// new STree (GP:1519): one leaf whose sampling tree is a single empty quadtree node
-static int init_tree(ppg_integrator *h) {
-    CK(h->dScalars.alloc(8)); CK(h->dTreeStats.alloc(1));
-    CK(cudaMemsetAsync(h->dScalars.p, 0, 32, h->stream));
-    // buffers persist across renders (cudaMalloc/cudaFree are synchronous and slow): only their contents are reset
-    int rc = ensure_tree_capacity(h, std::max<uint32_t>(h->capNodes, 1u << 16), std::max<size_t>(h->capPool, (size_t) 1 << 20));
-    if (rc) return rc;
-    CK(cudaMemsetAsync(h->dSnodes.p, 0, sizeof(uint2) * h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dLeafA.p, 0, sizeof(float4) * h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dBweight.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dSampSum.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dSampWeight.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dAdam.p, 0, 24 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dAdamCount.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dAdamCursor.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dSampDepth.p, 0, 4 * (size_t) h->capNodes, h->stream));
-    CK(cudaMemsetAsync(h->dSamp.p, 0, sizeof(SampNode), h->stream));          // one empty quadtree node at pool offset 0
-    const uint32_t one[2] = {1u, 1u};
-    CK(cudaMemcpyAsync(h->dScalars.p, one, 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->dSampCount.p, one, 4, cudaMemcpyHostToDevice, h->stream));
-    h->hNodes = 1; h->hTotalBuild = 1;
-    CK(cudaStreamSynchronize(h->stream));
-    return PPG_OK;
-}
-
-static TreeView tree_view(ppg_integrator *h) {
-    TreeView T;
-    T.snodes = h->dSnodes.p; T.stable = stree_table_usable(h->hNodes) ? h->dStable.p : nullptr; T.leafA = h->dLeafA.p; T.samp = h->dSamp.p; T.bchildren = h->dBchildren.p;
-    T.bsums = reinterpret_cast<float4 *>(h->dTrain.p); T.bweight = h->dBweight.p;
-    T.aabbMin = make_float3(h->aabbMin[0], h->aabbMin[1], h->aabbMin[2]); T.extent = make_float3(h->extent[0], h->extent[1], h->extent[2]);
-    return T;
-}
-
 // S-tree node capacity for a refine: a leaf splits only while its weight exceeds the threshold, so the refinement creates at most
 // 4 nodes per threshold worth of building weight
 static double refine_capacity(size_t nodes, double totalWeight, float threshold) { return (double) nodes + 4.0 * totalWeight / std::max(1.0f, threshold) + 1024; }
@@ -585,43 +724,22 @@ static int reset_sd_tree(ppg_integrator *h) {
     // the total weight of the last iteration bounds the number of new leaves by 2*W/threshold
     bool memCapped = false;
     if (h->prm.sd_tree_max_memory >= 0) {   // GP:958-967 (footprint approximated by node counts: 2 trees x 24 B per node + per-tree overhead)
-        const size_t fp = (size_t) h->hTotalBuild * 2 * 24 + (size_t) h->hNodes * 96;
+        const size_t fp = (size_t) h->tree.hTotalBuild * 2 * 24 + (size_t) h->tree.hNodes * 96;
         memCapped = fp / 1000000 >= (size_t) h->prm.sd_tree_max_memory;
     }
     if (!memCapped) {
         // capacity: the refinement creates at most 2 nodes per threshold worth of recorded weight.  The total weight of the iteration is at most
         // its number of guiding records (weights <= 1), summed over the ranks whose weights are reduced.
         const double totalW = 1.25 * (double) h->lastRecorded + 4096;
-        const double est = refine_capacity(h->hNodes, totalW, threshold);
-        int rc = ensure_tree_capacity(h, (uint32_t) std::min<double>(est, 4.0e9), h->capPool);
+        const double est = refine_capacity(h->tree.hNodes, totalW, threshold);
+        int rc = h->tree.reserve((uint32_t) std::min<double>(est, 4.0e9), h->tree.capPool);
         if (rc) return rc;
-        MaintParams M = maint(h);
-        h->tic(PPG_K_REFINE); stree_refine_kernel<<<1, 1024, 0, h->stream>>>(M, threshold, h->dScalars.p + 5); h->toc(); h->launches++;
+        h->tic(PPG_K_REFINE); h->launches += h->tree.refine(threshold); h->toc();
     }
-    MaintParams M = maint(h);
-    const int blocks = h->numSMs * 4;
-    h->tic(PPG_K_RESET);
-    dtree_reset_kernel<false><<<blocks, 128, 0, h->stream>>>(M, nullptr, 20, h->prm.d_tree_threshold); h->launches++;
-    exclusive_scan_kernel<<<1, 1024, 0, h->stream>>>(h->dBuildCount.p, h->dBuildBase.p, h->dScalars.p, h->dScalars.p + 1); h->launches++;
-    h->toc();
-    uint32_t sc[8];
-    CK(cudaMemcpyAsync(sc, h->dScalars.p, 32, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (sc[5]) return fail(PPG_ERR_CUDA, "S-tree refinement ran out of node capacity");
-    h->hNodes = sc[0]; h->hTotalBuild = sc[1];
-    int rc = ensure_tree_capacity(h, h->hNodes, std::max<size_t>(h->hTotalBuild, 1));
-    if (rc) return rc;
-    M = maint(h);
-    h->tic(PPG_K_RESET);
-    dtree_reset_kernel<true><<<blocks, 128, 0, h->stream>>>(M, h->dBuildBase.p, 20, h->prm.d_tree_threshold); h->launches++;
-    leaf_after_reset_kernel<<<blocks, 256, 0, h->stream>>>(M, h->dBuildBase.p); h->launches++;
-    h->toc();
-    // prefix table of the refined S-tree (stree_lookup): the first 3 * PPG_STREE_TABLE_BITS levels of every descent become one load.
-    // Past 0xFFFFFF nodes its entries cannot hold the node numbers: tree_view then hands out no table and the kernels walk from the root.
-    if (stree_table_usable(h->hNodes)) {
-        CK(h->dStable.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-        h->tic(PPG_K_REFINE); stree_table_kernel<<<h->numSMs * 8, 256, 0, h->stream>>>(h->dSnodes.p, h->dStable.p); h->toc(); h->launches++;
-    }
+    h->tic(PPG_K_RESET); h->launches += h->tree.reset_count(20, h->prm.d_tree_threshold); h->toc();
+    int rc = h->tree.sync_counts(); if (rc) return rc;
+    h->tic(PPG_K_RESET); h->launches += h->tree.reset_fill(20, h->prm.d_tree_threshold); h->toc();
+    if (stree_table_usable(h->tree.hNodes)) { h->tic(PPG_K_REFINE); h->launches += h->tree.stree_table(); h->toc(); }
     CK(cudaGetLastError());
     return PPG_OK;      // no synchronize: the passes queue behind the reset
 }
@@ -634,16 +752,16 @@ __global__ void pack_tail_kernel(float *tail, float *bweight, uint32_t n, int di
 }
 static int exchange_training_statistics(ppg_integrator *h) {
     if (!h->multi()) return PPG_OK;
-    float *tail = h->dTrain.p + 4 * (size_t) h->hTotalBuild;
-    pack_tail_kernel<<<h->numSMs, 256, 0, h->stream>>>(tail, h->dBweight.p, h->hNodes, 0); h->launches++;
-    int rc = allreduce_sum(h, h->dTrain.p, 4 * (size_t) h->hTotalBuild + (size_t) h->hNodes); if (rc) return rc;
-    pack_tail_kernel<<<h->numSMs, 256, 0, h->stream>>>(tail, h->dBweight.p, h->hNodes, 1); h->launches++;
+    float *tail = h->tree.dTrain.p + 4 * (size_t) h->tree.hTotalBuild;
+    pack_tail_kernel<<<h->numSMs, 256, 0, h->stream>>>(tail, h->tree.dBweight.p, h->tree.hNodes, 0); h->launches++;
+    int rc = allreduce_sum(h, h->tree.dTrain.p, 4 * (size_t) h->tree.hTotalBuild + (size_t) h->tree.hNodes); if (rc) return rc;
+    pack_tail_kernel<<<h->numSMs, 256, 0, h->stream>>>(tail, h->tree.dBweight.p, h->tree.hNodes, 1); h->launches++;
     return PPG_OK;
 }
 // a host scalar made identical on all ranks (rank 0's value wins): time-based decisions must not diverge
 static int sync_scalar(ppg_integrator *h, float *v) {
     if (!h->multi()) return PPG_OK;
-    float *slot = h->dTrain.p + h->dTrain.n - 16;
+    float *slot = h->tree.dTrain.p + h->tree.dTrain.n - 16;
     const float mine = h->rank == 0 ? *v : 0.f;
     CK(cudaMemcpyAsync(slot, &mine, 4, cudaMemcpyHostToDevice, h->stream));
     int rc = allreduce_sum(h, slot, 1); if (rc) return rc;
@@ -652,21 +770,18 @@ static int sync_scalar(ppg_integrator *h, float *v) {
     return PPG_OK;
 }
 
-// buildSDTree, GP:1115-1189
+// buildSDTree, GP:1115-1189, with its "Distribution statistics" (GP:1121-1186) reduced on the device: 64 bytes come back
 static int build_sd_tree(ppg_integrator *h, ppg_iteration_stats &st) {
     int rc = exchange_training_statistics(h);
     if (rc) return rc;
-    MaintParams M = maint(h);
-    h->tic(PPG_K_BUILD); dtree_build_kernel<<<h->numSMs * 4, 128, 0, h->stream>>>(M, h->dBuildBase.p); h->toc(); h->launches++;
+    h->tic(PPG_K_BUILD); h->launches += h->tree.build(); h->toc();
     CK(cudaGetLastError());
-    // "Distribution statistics" (GP:1121-1186): reduced on the device, 64 bytes come back
-    CK(cudaMemsetAsync(h->dTreeStats.p, 0, sizeof(TreeStats), h->stream));
-    tree_stats_kernel<<<1, 1024, 0, h->stream>>>(M, h->dTreeStats.p); h->launches++;
+    h->launches += h->tree.tree_stats();
     // the statistics are only reported: they go to pinned memory and are folded into ppg_stats after the render's last synchronize
     const int slot = std::min(h->iter, PPG_MAX_ITERATIONS - 1);
-    CK(cudaMemcpyAsync(h->hTreeStats + slot, h->dTreeStats.p, sizeof(TreeStats), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(h->hTreeStats + slot, h->tree.dTreeStats.p, sizeof(TreeStats), cudaMemcpyDeviceToHost, h->stream));
     h->treeStatsPending[slot] = true;
-    st.s_tree_nodes = h->hNodes;
+    st.s_tree_nodes = h->tree.hNodes;
     h->isBuilt = true;
     return PPG_OK;
 }
@@ -717,10 +832,10 @@ static int ensure_wavefront(ppg_integrator *h) {
         // lengths of the bundled scenes: 4 - 9 vertices; the spatial box filter touches ~2 leaves per vertex); a record beyond it is dropped and
         // counted in ppg_stats.dropped_records.  Allocating per batch (cudaMalloc / cudaFree are synchronous) cost 11 ms per sub-batch.
         const size_t want = cap * 16 * (h->prm.spatial_filter == PPG_SFILTER_BOX ? 2 : 1);
-        if (want > h->adamCap) {
-            h->dAdamRecA.release(); h->dAdamRecB.release(); h->dAdamSortA.release(); h->dAdamSortB.release();
-            CK(h->dAdamRecA.alloc(want)); CK(h->dAdamRecB.alloc(want)); CK(h->dAdamSortA.alloc(want)); CK(h->dAdamSortB.alloc(want));
-            h->adamCap = want;
+        if (want > h->tree.adamCap) {
+            h->tree.dAdamRecA.release(); h->tree.dAdamRecB.release(); h->tree.dAdamSortA.release(); h->tree.dAdamSortB.release();
+            CK(h->tree.dAdamRecA.alloc(want)); CK(h->tree.dAdamRecB.alloc(want)); CK(h->tree.dAdamSortA.alloc(want)); CK(h->tree.dAdamSortB.alloc(want));
+            h->tree.adamCap = want;
         }
     }
     // persistent grids: resident blocks per SM from the occupancy calculator
@@ -730,8 +845,6 @@ static int ensure_wavefront(ppg_integrator *h) {
     CK(cudaGetLastError());
     // one block per resident slot; warps claim their work dynamically (bounce_kernel)
     h->gridBounce = h->numSMs * std::max(occ, 1) * std::max(env_int("PPG_GRID_MULT", 1), 1);
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, commit_kernel<1>, PPG_BLOCK, 0));
-    h->gridCommit = h->numSMs * std::max(occ, 1);
     // Scenes walked through the BVH find their hits in a separate pass of persistent warps (ppg_trace.cu) whenever the wavefront is large enough
     // to pay for the second launch per depth; tiny learning sub-batches keep the fused kernel.  PPG_TRACE_MIN_PATHS=0 turns the pass off.
     h->gridTrace = 0;
@@ -778,13 +891,13 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
     const int lossMode = (record && h->isBuilt) ? h->prm.bsdf_sampling_fraction_loss : PPG_LOSS_NONE;       // GP:2152
     const bool useAdam = lossMode != PPG_LOSS_NONE;
     const bool neeSlabs = nee && h->doNee && h->prm.nee != PPG_NEE_ALWAYS;
-    if (useAdam) CK(cudaMemsetAsync(h->dScalars.p + 3, 0, 4, h->stream));      // record cursor (buffers: ensure_wavefront)
+    if (useAdam) CK(cudaMemsetAsync(h->tree.dScalars.p + 3, 0, 4, h->stream));      // record cursor (buffers: ensure_wavefront)
     if (nPaths) {
         CK(cudaMemsetAsync(h->dLive.p, 0, 4 * (size_t) (h->maxBounces + 2), h->stream));
         CK(cudaMemsetAsync(h->dWork.p, 0, 4 * (size_t) (h->maxBounces + 2), h->stream));
         CK(cudaMemcpyAsync(h->dLive.p, &nPaths, 4, cudaMemcpyHostToDevice, h->stream));
         RenderParams P;
-        P.scene = h->sceneView; P.cam = h->cam; P.tree = tree_view(h);
+        P.scene = h->sceneView; P.cam = h->cam; P.tree = h->tree.view(h->aabbMin, h->extent);
         P.liFinal = h->dLiFinal.p; P.pixelMap = pixelMap; P.counters = h->dCounters.p;
         P.nPaths = nPaths; P.nLocalPixels = pixelCount; P.spp = (uint32_t) h->prm.spp_per_pass;
         P.passBase = (uint64_t) h->passesRendered; P.seed = h->prm.seed;
@@ -841,18 +954,14 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
         }
         if (record) {
             CommitParams C;
-            C.tree = tree_view(h); C.slab0 = slab_at(h, 0); C.slabStride = h->pathCapacity; C.liveCounts = h->dLive.p; C.liFinal = h->dLiFinal.p;
+            C.tree = h->tree.view(h->aabbMin, h->extent); C.slab0 = slab_at(h, 0); C.slabStride = h->pathCapacity; C.liveCounts = h->dLive.p; C.liFinal = h->dLiFinal.p;
             C.spatialFilter = h->prm.spatial_filter; C.directionalFilter = h->prm.directional_filter;
             C.lossMode = lossMode;
             C.statisticalWeight = (h->prm.nee == PPG_NEE_KICKSTART && h->doNee && nee) ? 0.5f : 1.0f;   // GP:2152
-            C.seed = h->prm.seed; C.snodes = h->dSnodes.p; C.nSlabs = (uint32_t) std::min(h->nSlabs, lastDepth);
+            C.seed = h->prm.seed; C.nSlabs = (uint32_t) std::min(h->nSlabs, lastDepth);
             C.nee0 = neeSlabs ? slab_at(h, 0, 1) : C.slab0;
-            C.adamRecA = h->dAdamRecA.p; C.adamRecB = h->dAdamRecB.p; C.adamTotal = h->dScalars.p + 3; C.adamCap = (uint32_t) std::min<size_t>(h->adamCap, 0xFFFFFFFFu);
             C.dropped = h->dCounters.p + 4;
-            dim3 g(std::min<int>(h->gridCommit, (int) ((nPaths + PPG_BLOCK - 1) / PPG_BLOCK)), C.nSlabs * (neeSlabs ? 2 : 1));
-            h->tic(PPG_K_COMMIT);
-            if (record == 1) commit_kernel<1><<<g, PPG_BLOCK, 0, h->stream>>>(C); else commit_kernel<2><<<g, PPG_BLOCK, 0, h->stream>>>(C);
-            h->toc(); h->launches++;
+            h->tic(PPG_K_COMMIT); h->launches += h->tree.commit(C, record, nPaths, C.nSlabs * (neeSlabs ? 2 : 1)); h->toc();
         }
         h->tic(PPG_K_FILM);
         film_kernel<<<std::min<int>(h->numSMs * 8, (int) ((pixelCount + PPG_BLOCK - 1) / PPG_BLOCK)), PPG_BLOCK, 0, h->stream>>>(
@@ -861,30 +970,22 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
     }
     if (useAdam) {
         // replay the sampling-fraction records leaf by leaf (see adam_seq_kernel)
-        MaintParams M = maint(h);
+        const MaintParams M = h->tree.maint();
         const bool multi = h->multi();
-        float *tail = h->dTrain.p + 4 * (size_t) h->hTotalBuild;       // [6 x nNodes] exchange area (the building weights are packed there only at iteration end)
-        adam_pack_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, nullptr, 0); h->launches++;
-        h->tic(PPG_K_OTHER);      // bucket the records by leaf (histogram, scan, scatter): "other"; the sequential replay itself: "adam"
-        adam_hist_kernel<<<h->numSMs * 4, 256, 0, h->stream>>>(h->dAdamRecA.p, h->dScalars.p + 3, (uint32_t) h->adamCap, h->dAdamCount.p); h->launches++;
-        exclusive_scan_kernel<<<1, 1024, 0, h->stream>>>(h->dAdamCount.p, h->dAdamOffset.p, h->dScalars.p, h->dScalars.p + 4); h->launches++;
-        adam_scatter_kernel<<<h->numSMs * 4, 256, 0, h->stream>>>(h->dAdamRecA.p, h->dAdamRecB.p, h->dScalars.p + 3, (uint32_t) h->adamCap, h->dAdamOffset.p,
-                                                                  h->dAdamCursor.p, h->dAdamSortA.p, h->dAdamSortB.p); h->launches++;
-        h->toc();
-        h->tic(PPG_K_ADAM);
-        adam_seq_kernel<<<h->numSMs * 16, 128, 0, h->stream>>>(M, h->dAdamSortA.p, h->dAdamSortB.p, h->dAdamOffset.p, h->dAdamCount.p, h->dAdamCursor.p,
-                                                              lossMode == PPG_LOSS_KL ? 1.0f : 2.0f); h->launches++;
-        h->toc();
+        float *tail = h->tree.dTrain.p + 4 * (size_t) h->tree.hTotalBuild;       // [6 x nNodes] exchange area (the building weights are packed there only at iteration end)
+        adam_pack_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->tree.dAdamBefore.p, nullptr, 0); h->launches++;
+        h->tic(PPG_K_OTHER); h->launches += h->tree.adam_bucket(); h->toc();      // bucket the records by leaf (histogram, scan, scatter): "other"
+        h->tic(PPG_K_ADAM); h->launches += h->tree.adam_replay(lossMode); h->toc();      // the sequential replay itself: "adam"
         if (multi) {
             // replicas replayed their own records from the common state: merge them (steps and moves of the variable add up, moments are
             // weighted by the steps, batch accumulators add up relative to the common start) so that all ranks continue identically
-            adam_pack_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, nullptr, 1); h->launches++;
-            int rc = allreduce_sum(h, tail, 6 * (size_t) h->hNodes); if (rc) return rc;
-            adam_merge_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->dAdamBefore.p, (float) (h->world - 1)); h->launches++;
+            adam_pack_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->tree.dAdamBefore.p, nullptr, 1); h->launches++;
+            int rc = allreduce_sum(h, tail, 6 * (size_t) h->tree.hNodes); if (rc) return rc;
+            adam_merge_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, tail, h->tree.dAdamBefore.p, (float) (h->world - 1)); h->launches++;
         }
         // movement of the fractions in this replay (identical on all ranks after the merge): steers the size of the next sub-batch
         CK(cudaMemsetAsync(h->dCounters.p + 6, 0, 16, h->stream));
-        adam_progress_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, h->dAdamBefore.p, h->dCounters.p + 6); h->launches++;
+        adam_progress_kernel<<<h->numSMs, 256, 0, h->stream>>>(M, h->tree.dAdamBefore.p, h->dCounters.p + 6); h->launches++;
         CK(cudaMemcpyAsync(h->adamProgress, h->dCounters.p + 6, 16, cudaMemcpyDeviceToHost, h->stream));
     }
     CK(cudaGetLastError());
@@ -916,7 +1017,7 @@ static int perform_render_passes(ppg_integrator *h, float &variance, int numPass
     static const double growthMax = std::max(env_int("PPG_LOSS_GROWTH_MAX_PCT", 100), 1) * 0.01;
     static const double leafPaths = std::max(env_int("PPG_LOSS_LEAF_PATHS_X10", 40), 1) * 0.1;   // paths per S-tree leaf in the first sub-batch
     const double pathsPerPass = (double) npx * h->prm.spp_per_pass;                                  // whole image
-    const double minFrac = std::min(1.0, std::max(256.0, leafPaths * 0.5 * (h->hNodes + 1)) / std::max(pathsPerPass, 1.0));
+    const double minFrac = std::min(1.0, std::max(256.0, leafPaths * 0.5 * (h->tree.hNodes + 1)) / std::max(pathsPerPass, 1.0));
     double done = 0.0, frac = 0.0;          // passes rendered in this call (real number), fraction of the pass in progress
     double want = learning ? minFrac : (double) maxBatch, lastSize = 0.0;
     int local = 0; int rcode = PPG_OK;
@@ -973,7 +1074,7 @@ static int perform_render_passes(ppg_integrator *h, float &variance, int numPass
         variance_kernel<<<std::min<int>(h->numSMs * 4, (int) ((h->nLocalPixels + PPG_BLOCK - 1) / PPG_BLOCK)), PPG_BLOCK, 0, h->stream>>>(
             h->dImage.p, h->dSqImage.p, h->dPixelMap.p, h->nLocalPixels, h->W, (float) N, h->dVar.p);
     h->launches++;
-    float *slot = h->dTrain.p + h->dTrain.n - 16;
+    float *slot = h->tree.dTrain.p + h->tree.dTrain.n - 16;
     iteration_scalars_kernel<<<1, 1, 0, h->stream>>>(h->dVar.p, h->dCounters.p, slot); h->launches++;
     if (h->multi()) { int rc = allreduce_sum(h, slot, 2); if (rc) return rc; }
     float reduced[2] = {0, 0}; unsigned long long cnt[8];
@@ -1118,7 +1219,7 @@ static int ppg_render_device_impl(ppg_integrator *h, float **rgb_dev, ppg_stats 
     memset(&h->stats, 0, sizeof(h->stats)); h->launches = 0; h->deviceMs = 0; h->evUsed = 0;
     memset(h->treeStatsPending, 0, sizeof(h->treeStatsPending));
     CK(cudaEventRecord(h->evRender0, h->stream));
-    int rc = init_tree(h); if (rc) return rc;                                   // m_sdTree = new STree(scene->getAABB()), GP:1519
+    int rc = h->tree.init(); if (rc) return rc;                                   // m_sdTree = new STree(scene->getAABB()), GP:1519
     rc = ensure_wavefront(h); if (rc) return rc;
     h->iter = 0; h->isFinalIter = false; h->isBuilt = false; h->passesRendered = 0;
     for (auto *b : h->images) delete b;
@@ -1183,40 +1284,10 @@ extern "C" int ppg_get_moment_images(ppg_integrator *h, float *sum_rgbw, float *
     return PPG_OK;
 }
 
-// The integrator's SD-tree on the host: the S-tree and, per node, either the sampling trees (which == 0: the trees the passes guide with) or the
-// building trees (which == 1: the trees the passes record into).  Between the reset and the build of an iteration (the film callback) the sampling
-// trees still sit where the previous build put them, past the new building total: the copy of the quadtree pool is sized from the leaves.
-struct TreeGather {
-    uint32_t n = 0;
-    std::vector<uint2> sn; std::vector<float4> la; std::vector<float> sum, weight, adam; std::vector<int> depth; std::vector<uint32_t> count;
-    std::vector<uint2> children; std::vector<float4> sums;      // the quadtree pool from offset 0 (building: bchildren / bsums; sampling: dSamp)
-    uint32_t first(uint32_t i, int which) const { uint32_t u; memcpy(&u, which ? &la[i].y : &la[i].x, 4); return u; }
-};
 static int gather_tree(ppg_integrator *h, int which, TreeGather &g) {
-    if (!h->haveScene || h->capNodes == 0) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
+    if (!h->haveScene) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
     CK(cudaSetDevice(h->device));
-    const uint32_t n = g.n = h->hNodes;
-    g.sn.resize(n); g.la.resize(n); g.sum.assign(n, 0.f); g.weight.resize(n); g.adam.resize(6 * (size_t) n); g.depth.resize(n); g.count.resize(n);
-    CK(cudaMemcpy(g.sn.data(), h->dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(g.la.data(), h->dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(g.adam.data(), h->dAdam.p, 24 * (size_t) n, cudaMemcpyDeviceToHost));
-    if (which == 0) CK(cudaMemcpy(g.sum.data(), h->dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(g.weight.data(), which ? h->dBweight.p : h->dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(g.depth.data(), which ? h->dBuildDepth.p : h->dSampDepth.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(g.count.data(), which ? h->dBuildCount.p : h->dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-    size_t end = 1;
-    for (uint32_t i = 0; i < n; ++i) if (g.sn[i].x == 0u) end = std::max<size_t>(end, (size_t) g.first(i, which) + g.count[i]);
-    if (end > h->capPool) return fail(PPG_ERR_CUDA, "SD-tree leaf points past the quadtree pool");
-    g.children.resize(end); g.sums.resize(end);
-    if (which) {
-        CK(cudaMemcpy(g.children.data(), h->dBchildren.p, sizeof(uint2) * end, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.sums.data(), h->dTrain.p, sizeof(float4) * end, cudaMemcpyDeviceToHost));
-    } else {
-        std::vector<SampNode> pool(end);
-        CK(cudaMemcpy(pool.data(), h->dSamp.p, sizeof(SampNode) * end, cudaMemcpyDeviceToHost));
-        for (size_t k = 0; k < end; ++k) { g.children[k] = pool[k].children; g.sums[k] = pool[k].sums; }
-    }
-    return PPG_OK;
+    return h->tree.gather(which, g);
 }
 
 extern "C" int ppg_export_sdtree(ppg_integrator *h, int which, size_t node_capacity, size_t *n_nodes_out, uint32_t *node_children, uint64_t *tree_first,
@@ -1384,15 +1455,6 @@ static int op_device(int device) {
     CK(cudaSetDevice(device));
     return PPG_OK;
 }
-static std::vector<SampNode> to_pool(const float *sums, const uint16_t *children, size_t n) {
-    std::vector<SampNode> pool(n);
-    for (size_t i = 0; i < n; ++i) {
-        pool[i].sums = make_float4(sums[4 * i], sums[4 * i + 1], sums[4 * i + 2], sums[4 * i + 3]);
-        pool[i].children = make_uint2((uint32_t) children[4 * i] | ((uint32_t) children[4 * i + 1] << 16), (uint32_t) children[4 * i + 2] | ((uint32_t) children[4 * i + 3] << 16));
-        pool[i].pad = make_uint2(0u, 0u);
-    }
-    return pool;
-}
 }  // namespace
 
 extern "C" int ppg_op_dtree_pdf(int device, const float *sums, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
@@ -1494,34 +1556,25 @@ extern "C" int ppg_op_env_pdf(ppg_integrator *h, size_t n, const float *d, float
 }
 extern "C" int ppg_op_stree_lookup(int device, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
                                    const float *points, size_t n, uint32_t *leaf_out, float *size_out) {
+  return guarded("ppg_op_stree_lookup", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    Up<uint2> dn; Up<float> dp; DevBuf<uint32_t> dl; DevBuf<float> dsz;
-    if (dn.up(reinterpret_cast<const uint2 *>(node_children), n_nodes) || dp.up(points, 3 * n)) return fail(PPG_ERR_CUDA, "upload failed");
+    if (n_nodes >= 0xFFFFFFFFull) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_stree_lookup: more S-tree nodes than 32-bit node numbers hold");
+    TreeStore t;
+    rc = t.load(0, n_nodes, (uint32_t) n_nodes, node_children, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr); if (rc) return rc;
+    Up<float> dp; DevBuf<uint32_t> dl; DevBuf<float> dsz;
+    if (dp.up(points, 3 * n)) return fail(PPG_ERR_CUDA, "upload failed");
     CK(dl.alloc(std::max<size_t>(n, 1))); CK(dsz.alloc(std::max<size_t>(3 * n, 1)));
-    DevBuf<uint32_t> dt;
-    if (stree_table_usable(n_nodes)) {                    // the same prefix table the render kernels use, under the same rule
-        CK(dt.alloc((size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-        stree_table_kernel<<<296, 256>>>(dn.b.p, dt.p);
-    }
-    if (n) op_lookup_kernel<<<296, 256>>>(dn.b.p, dt.p,make_float3(aabb_min[0], aabb_min[1], aabb_min[2]), make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]), dp.b.p, n, dl.p, dsz.p);
+    t.stree_table();
+    const TreeView T = t.view(aabb_min, aabb_extent);
+    if (n) op_lookup_kernel<<<t.numSMs * 2, 256>>>(T.snodes, T.stable, T.aabbMin, T.extent, dp.b.p, n, dl.p, dsz.p);
     CK(cudaGetLastError());
     CK(cudaMemcpy(leaf_out, dl.p, 4 * n, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(size_out, dsz.p, 12 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
+  });
 }
 
-// ------------------------------------------------------------------ the learning half: the render's own maintenance, commit and Adam kernels
-namespace {
-static float bits_f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
-static uint32_t f_bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
-static int op_sm_count() { int d = 0, n = 0; if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) != cudaSuccess) n = 132; return n; }
-// a zero-filled device array of `cap` elements whose first n are copied from the host (host may be null: zeros)
-template <class T> static cudaError_t dev_array(DevBuf<T> &b, size_t cap, const T *host = nullptr, size_t n = 0) {
-    cudaError_t e = b.alloc(std::max<size_t>(cap, 1)); if (e != cudaSuccess) return e;
-    e = cudaMemset(b.p, 0, std::max<size_t>(cap, 1) * sizeof(T)); if (e != cudaSuccess) return e;
-    return (host && n) ? cudaMemcpy(b.p, host, n * sizeof(T), cudaMemcpyHostToDevice) : cudaSuccess;
-}
-}  // namespace
+// ------------------------------------------------------------------ the learning half: the render's own maintenance, commit and Adam launches (TreeStore)
 
 extern "C" int ppg_op_sdtree_refine_reset(int device, int stages, float threshold, int new_max_depth, float dtree_threshold, size_t node_capacity,
                                           const uint32_t *node_children, size_t n_nodes, const uint32_t *tree_first, const uint32_t *tree_count, const int32_t *tree_depth,
@@ -1540,55 +1593,33 @@ extern "C" int ppg_op_sdtree_refine_reset(int device, int stages, float threshol
     const uint32_t cap = node_capacity ? (uint32_t) std::min<size_t>(node_capacity, 0xFFFFFFFFull)
                                        : std::max<uint32_t>((uint32_t) std::min<double>(refine_capacity(n_nodes, 1.25 * totalW + 4096, threshold), 4.0e9), 1u << 16);
     if (cap < n_nodes) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: node_capacity below n_nodes");
-    std::vector<float4> la(n_nodes);
-    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(tree_first[i]), 0.f, adam[6 * i + 3], 0.f);
-    std::vector<SampNode> pool = to_pool(sums, children, n_pool);
-    DevBuf<uint2> dS, dBch; DevBuf<float4> dLA, dBs; DevBuf<float> dBW, dSS, dSW, dAd; DevBuf<int> dSD, dBD; DevBuf<uint32_t> dSC, dBC, dBB, dSc; DevBuf<SampNode> dSamp;
-    CK(dev_array(dS, cap, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, cap, la.data(), n_nodes));
-    CK(dev_array(dBW, cap, building_weight, n_nodes)); CK(dev_array(dSS, cap, tree_sum, n_nodes)); CK(dev_array(dSW, cap, tree_weight, n_nodes));
-    CK(dev_array(dSD, cap, tree_depth, n_nodes)); CK(dev_array(dSC, cap, tree_count, n_nodes)); CK(dev_array(dAd, 6 * (size_t) cap, adam, 6 * n_nodes));
-    CK(dev_array(dBC, cap)); CK(dev_array(dBD, cap)); CK(dev_array(dBB, cap)); CK(dev_array(dSamp, n_pool, pool.data(), n_pool));
-    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, 0, 0, 0, 0, 0};
-    CK(dev_array(dSc, 8, sc0, 8));
-    MaintParams M;
-    M.snodes = dS.p; M.leafA = dLA.p; M.bweight = dBW.p; M.sampSum = dSS.p; M.sampWeight = dSW.p; M.sampDepth = dSD.p; M.sampCount = dSC.p; M.adam = dAd.p;
-    M.buildCount = dBC.p; M.buildDepth = dBD.p; M.nNodes = dSc.p; M.capNodes = cap; M.samp = dSamp.p; M.bchildren = nullptr; M.bsums = nullptr;
-    if (stages & 1) stree_refine_kernel<<<1, 1024>>>(M, threshold, dSc.p + 5);        // launch shapes of reset_sd_tree
+    TreeStore t;
+    rc = t.load(0, n_nodes, cap, node_children, tree_first, tree_count, tree_depth, tree_sum, tree_weight, adam, n_pool, sums, children); if (rc) return rc;
+    CK(t.put(t.dBweight, building_weight, n_nodes));
+    if (stages & 1) t.refine(threshold);
+    if (stages & 2) t.reset_count(new_max_depth, dtree_threshold);
     CK(cudaGetLastError());
-    uint32_t hs[8]; CK(cudaMemcpy(hs, dSc.p, 32, cudaMemcpyDeviceToHost));
-    if (hs[5]) return fail(PPG_ERR_CUDA, "S-tree refinement ran out of node capacity");
-    const size_t N = hs[0];
-    std::vector<float> bwRefined(N); CK(cudaMemcpy(bwRefined.data(), dBW.p, 4 * N, cudaMemcpyDeviceToHost));      // leaf_after_reset_kernel zeroes it
-    size_t total = 0;
-    if (stages & 2) {
-        const int blocks = op_sm_count() * 4;
-        dtree_reset_kernel<false><<<blocks, 128>>>(M, nullptr, new_max_depth, dtree_threshold);
-        exclusive_scan_kernel<<<1, 1024>>>(dBC.p, dBB.p, dSc.p, dSc.p + 1);
-        CK(cudaGetLastError());
-        CK(cudaMemcpy(hs, dSc.p, 32, cudaMemcpyDeviceToHost)); total = hs[1];
-        CK(dev_array(dBch, total)); CK(dev_array(dBs, total));
-        M.bchildren = dBch.p; M.bsums = dBs.p;
-        dtree_reset_kernel<true><<<blocks, 128>>>(M, dBB.p, new_max_depth, dtree_threshold);
-        leaf_after_reset_kernel<<<blocks, 256>>>(M, dBB.p);
-        CK(cudaGetLastError());
-    }
+    rc = t.sync_counts(true); if (rc) return rc;
+    const size_t N = t.hNodes, total = t.hTotalBuild;
     *n_nodes_out = N; *n_build_out = total;
     if (N > out_capacity || total > build_capacity)
         return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: output arrays too small (*n_nodes_out and *n_build_out hold the sizes needed)");
-    std::vector<float4> laOut(N); CK(cudaMemcpy(laOut.data(), dLA.p, 16 * N, cudaMemcpyDeviceToHost));
+    if (building_weight_out) CK(cudaMemcpy(building_weight_out, t.dBweight.p, 4 * N, cudaMemcpyDeviceToHost));      // reset_fill zeroes it
+    if (stages & 2) t.reset_fill(new_max_depth, dtree_threshold);
+    CK(cudaGetLastError());
+    std::vector<float4> laOut(N); CK(cudaMemcpy(laOut.data(), t.dLeafA.p, 16 * N, cudaMemcpyDeviceToHost));
     if (tree_first_out) for (size_t i = 0; i < N; ++i) tree_first_out[i] = f_bits(laOut[i].x);
-    if (node_children_out) CK(cudaMemcpy(node_children_out, dS.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (tree_count_out) CK(cudaMemcpy(tree_count_out, dSC.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, dSD.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, dSS.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, dSW.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (adam_out) CK(cudaMemcpy(adam_out, dAd.p, 24 * N, cudaMemcpyDeviceToHost));
-    if (building_weight_out) memcpy(building_weight_out, bwRefined.data(), 4 * N);
-    if (build_first_out) CK(cudaMemcpy(build_first_out, dBB.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_count_out) CK(cudaMemcpy(build_count_out, dBC.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_depth_out) CK(cudaMemcpy(build_depth_out, dBD.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_children_out && total) CK(cudaMemcpy(build_children_out, dBch.p, 8 * total, cudaMemcpyDeviceToHost));     // uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
-    if (build_sums_out && total) CK(cudaMemcpy(build_sums_out, dBs.p, 16 * total, cudaMemcpyDeviceToHost));
+    if (node_children_out) CK(cudaMemcpy(node_children_out, t.dSnodes.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (tree_count_out) CK(cudaMemcpy(tree_count_out, t.dSampCount.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, t.dSampDepth.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, t.dSampSum.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, t.dSampWeight.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (adam_out) CK(cudaMemcpy(adam_out, t.dAdam.p, 24 * N, cudaMemcpyDeviceToHost));
+    if (build_first_out) CK(cudaMemcpy(build_first_out, t.dBuildBase.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_count_out) CK(cudaMemcpy(build_count_out, t.dBuildCount.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_depth_out) CK(cudaMemcpy(build_depth_out, t.dBuildDepth.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (build_children_out && total) CK(cudaMemcpy(build_children_out, t.dBchildren.p, 8 * total, cudaMemcpyDeviceToHost));     // uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
+    if (build_sums_out && total) CK(cudaMemcpy(build_sums_out, t.dTrain.p, 16 * total, cudaMemcpyDeviceToHost));
     return PPG_OK;
   });
 }
@@ -1601,40 +1632,22 @@ extern "C" int ppg_op_sdtree_build(int device, const uint32_t *node_children, si
     int rc = op_device(device); if (rc) return rc;
     if (!n_nodes || n_nodes >= 0xFFFFFFFFull || !node_children || !build_first || !build_count || !build_depth || !building_weight || !sums || !children || !n_pool)
         return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_build: empty or null input");
-    std::vector<float4> la(n_nodes);
-    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(build_first[i]), bits_f(build_first[i]), 0.f, 0.f);
-    DevBuf<uint2> dS, dBch; DevBuf<float4> dLA, dBs; DevBuf<float> dBW, dSS, dSW; DevBuf<int> dSD, dBD; DevBuf<uint32_t> dSC, dBC, dBB, dSc; DevBuf<SampNode> dSamp;
-    DevBuf<TreeStats> dTS;
-    CK(dev_array(dS, n_nodes, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, n_nodes, la.data(), n_nodes));
-    CK(dev_array(dBW, n_nodes, building_weight, n_nodes)); CK(dev_array(dSS, n_nodes)); CK(dev_array(dSW, n_nodes)); CK(dev_array(dSD, n_nodes)); CK(dev_array(dSC, n_nodes));
-    CK(dev_array(dBC, n_nodes, build_count, n_nodes)); CK(dev_array(dBD, n_nodes, build_depth, n_nodes)); CK(dev_array(dBB, n_nodes, build_first, n_nodes));
-    CK(dev_array(dBch, n_pool, reinterpret_cast<const uint2 *>(children), n_pool)); CK(dev_array(dBs, n_pool, reinterpret_cast<const float4 *>(sums), n_pool));
-    CK(dev_array(dSamp, n_pool)); CK(dev_array(dTS, 1));
-    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, 0, 0, 0, 0, 0};
-    CK(dev_array(dSc, 8, sc0, 8));
-    MaintParams M;
-    M.snodes = dS.p; M.leafA = dLA.p; M.bweight = dBW.p; M.sampSum = dSS.p; M.sampWeight = dSW.p; M.sampDepth = dSD.p; M.sampCount = dSC.p; M.adam = nullptr;
-    M.buildCount = dBC.p; M.buildDepth = dBD.p; M.nNodes = dSc.p; M.capNodes = (uint32_t) n_nodes; M.samp = dSamp.p; M.bchildren = dBch.p; M.bsums = dBs.p;
-    dtree_build_kernel<<<op_sm_count() * 4, 128>>>(M, dBB.p);        // launch shapes of build_sd_tree
-    tree_stats_kernel<<<1, 1024>>>(M, dTS.p);
+    TreeStore t; rc = t.load(1, n_nodes, (uint32_t) n_nodes, node_children, build_first, build_count, build_depth, nullptr, building_weight, nullptr, n_pool, sums, children);
+    if (rc) return rc;
+    t.build(); t.tree_stats();
     CK(cudaGetLastError());
-    std::vector<SampNode> pool(n_pool); CK(cudaMemcpy(pool.data(), dSamp.p, sizeof(SampNode) * n_pool, cudaMemcpyDeviceToHost));
-    for (size_t k = 0; k < n_pool; ++k) {
-        if (sampling_sums_out) memcpy(sampling_sums_out + 4 * k, &pool[k].sums, 16);
-        if (sampling_children_out) memcpy(sampling_children_out + 4 * k, &pool[k].children, 8);
-    }
-    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, dSS.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, dSW.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, dSD.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    if (tree_count_out) CK(cudaMemcpy(tree_count_out, dSC.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    if (mean_positive_out) {
-        std::vector<float4> laOut(n_nodes); CK(cudaMemcpy(laOut.data(), dLA.p, 16 * n_nodes, cudaMemcpyDeviceToHost));
-        for (size_t i = 0; i < n_nodes; ++i) mean_positive_out[i] = f_bits(laOut[i].w) != 0u;
-    }
+    TreeGather g; rc = t.gather(0, g, n_pool); if (rc) return rc;
+    if (sampling_sums_out) memcpy(sampling_sums_out, g.sums.data(), 16 * n_pool);
+    if (sampling_children_out) memcpy(sampling_children_out, g.children.data(), 8 * n_pool);
+    if (tree_sum_out) memcpy(tree_sum_out, g.sum.data(), 4 * n_nodes);
+    if (tree_weight_out) memcpy(tree_weight_out, g.weight.data(), 4 * n_nodes);
+    if (tree_depth_out) memcpy(tree_depth_out, g.depth.data(), 4 * n_nodes);
+    if (tree_count_out) memcpy(tree_count_out, g.count.data(), 4 * n_nodes);
+    if (mean_positive_out) for (size_t i = 0; i < n_nodes; ++i) mean_positive_out[i] = f_bits(g.la[i].w) != 0u;
     if (stats_out) {
-        TreeStats t; CK(cudaMemcpy(&t, dTS.p, sizeof(t), cudaMemcpyDeviceToHost));
-        const double v[14] = {(double) t.leaves, (double) t.leavesWithNodes, (double) t.depthMin, (double) t.depthMax, t.meanMin, t.meanMax, t.weightMin, t.weightMax,
-                              (double) t.nodesMin, (double) t.nodesMax, t.depthSum, t.meanSum, t.nodesSum, t.weightSum};
+        TreeStats s; CK(cudaMemcpy(&s, t.dTreeStats.p, sizeof(s), cudaMemcpyDeviceToHost));
+        const double v[14] = {(double) s.leaves, (double) s.leavesWithNodes, (double) s.depthMin, (double) s.depthMax, s.meanMin, s.meanMax, s.weightMin, s.weightMax,
+                              (double) s.nodesMin, (double) s.nodesMax, s.depthSum, s.meanSum, s.nodesSum, s.weightSum};
         memcpy(stats_out, v, sizeof(v));
     }
     return PPG_OK;
@@ -1651,47 +1664,35 @@ extern "C" int ppg_op_commit(int device, int record_mode, const uint32_t *node_c
     if (!n_nodes || !node_children || !aabb_min || !aabb_extent || !build_first || !building_weight_inout || !sums_inout || !children || !n_pool ||
         (n && (!vertices || !li_final)) || n >= 0x40000000ull || !n_adam_out)
         return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_commit: empty or null input");
-    std::vector<float4> la(n_nodes);
-    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(bits_f(build_first[i]), bits_f(build_first[i]), 0.f, 0.f);
+    TreeStore t; rc = t.load(1, n_nodes, (uint32_t) n_nodes, node_children, build_first, nullptr, nullptr, nullptr, building_weight_inout, nullptr, n_pool, sums_inout, children);
+    if (rc) return rc;
+    t.adamCap = std::min<size_t>(adam_capacity, 0xFFFFFFFFull); CK(t.dAdamRecA.alloc(t.adamCap)); CK(t.dAdamRecB.alloc(t.adamCap));
     // the bounce kernel's slab layout: field f of vertex i at f * n + i
     std::vector<float4> slab(6 * std::max<size_t>(n, 1));
     for (size_t i = 0; i < n; ++i)
         for (int f = 0; f < 6; ++f) memcpy(&slab[(size_t) f * n + i], vertices + 24 * i + 4 * f, 16);
-    const uint32_t live = (uint32_t) n, cap = (uint32_t) std::min<size_t>(adam_capacity, 0xFFFFFFFFull);
-    DevBuf<uint2> dS, dBch; DevBuf<uint32_t> dTab, dLive, dTot; DevBuf<float4> dLA, dBs, dSlab, dLi, dRA; DevBuf<float> dBW; DevBuf<float2> dRB; DevBuf<unsigned long long> dDrop;
-    CK(dev_array(dS, n_nodes, reinterpret_cast<const uint2 *>(node_children), n_nodes)); CK(dev_array(dLA, n_nodes, la.data(), n_nodes));
-    CK(dev_array(dBW, n_nodes, building_weight_inout, n_nodes));
-    CK(dev_array(dBch, n_pool, reinterpret_cast<const uint2 *>(children), n_pool)); CK(dev_array(dBs, n_pool, reinterpret_cast<const float4 *>(sums_inout), n_pool));
-    CK(dev_array(dSlab, slab.size(), slab.data(), slab.size())); CK(dev_array(dLi, n_li, reinterpret_cast<const float4 *>(li_final), n_li));
-    CK(dev_array(dLive, 1, &live, 1)); CK(dev_array(dTot, 1)); CK(dev_array(dDrop, 1)); CK(dev_array(dRA, cap)); CK(dev_array(dRB, cap));
-    if (stree_table_usable(n_nodes)) {                      // as after every refine (reset_sd_tree)
-        CK(dev_array(dTab, (size_t) 1 << (3 * PPG_STREE_TABLE_BITS)));
-        stree_table_kernel<<<296, 256>>>(dS.p, dTab.p);
-    }
+    const uint32_t live = (uint32_t) n; const unsigned long long dropped = 0;
+    Up<float4> dSlab, dLi; Up<uint32_t> dLive; Up<unsigned long long> dDrop;
+    if (dSlab.up(slab.data(), slab.size()) || dLi.up(reinterpret_cast<const float4 *>(li_final), n_li) || dLive.up(&live, 1) || dDrop.up(&dropped, 1))
+        return fail(PPG_ERR_CUDA, "upload failed");
+    t.stree_table();
     CommitParams C; memset(&C, 0, sizeof(C));
-    C.tree.snodes = dS.p; C.tree.stable = dTab.p; C.tree.leafA = dLA.p; C.tree.samp = nullptr; C.tree.bchildren = dBch.p; C.tree.bsums = dBs.p; C.tree.bweight = dBW.p;
-    C.tree.aabbMin = make_float3(aabb_min[0], aabb_min[1], aabb_min[2]); C.tree.extent = make_float3(aabb_extent[0], aabb_extent[1], aabb_extent[2]);
-    VertexSlab S; float4 *b = dSlab.p;
+    C.tree = t.view(aabb_min, aabb_extent);
+    VertexSlab S; float4 *b = dSlab.b.p;
     S.v0 = b; S.v1 = b + n; S.v2 = b + 2 * n; S.v3 = b + 3 * n; S.v4 = b + 4 * n; S.v5 = b + 5 * n;
-    C.slab0 = S; C.slabStride = n; C.liveCounts = dLive.p; C.liFinal = dLi.p;
+    C.slab0 = S; C.slabStride = n; C.liveCounts = dLive.b.p; C.liFinal = dLi.b.p;
     C.spatialFilter = spatial_filter; C.directionalFilter = directional_filter; C.lossMode = loss; C.statisticalWeight = statistical_weight;
-    C.nee0 = S; C.nSlabs = 1; C.seed = seed; C.snodes = dS.p;
-    C.adamRecA = dRA.p; C.adamRecB = dRB.p; C.adamTotal = dTot.p; C.adamCap = cap; C.dropped = dDrop.p;
-    if (n) {
-        int occ = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, commit_kernel<1>, PPG_BLOCK, 0));       // grid of render_batch
-        const dim3 g(std::min<int>(op_sm_count() * std::max(occ, 1), (int) ((n + PPG_BLOCK - 1) / PPG_BLOCK)), 1);
-        if (record_mode == 1) commit_kernel<1><<<g, PPG_BLOCK>>>(C); else commit_kernel<2><<<g, PPG_BLOCK>>>(C);
-    }
+    C.nee0 = S; C.nSlabs = 1; C.seed = seed; C.dropped = dDrop.b.p;
+    if (n) t.commit(C, record_mode, live, 1);
     CK(cudaGetLastError());
-    CK(cudaMemcpy(sums_inout, dBs.p, 16 * n_pool, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(building_weight_inout, dBW.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    uint32_t tot = 0; CK(cudaMemcpy(&tot, dTot.p, 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(sums_inout, t.dTrain.p, 16 * n_pool, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(building_weight_inout, t.dBweight.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    uint32_t tot = 0; CK(cudaMemcpy(&tot, t.dScalars.p + 3, 4, cudaMemcpyDeviceToHost));
     *n_adam_out = tot;
-    const size_t kept = std::min<size_t>(tot, cap);
+    const size_t kept = std::min<size_t>(tot, t.adamCap);
     if (adam_records_out && kept) {
         std::vector<float4> ra(kept); std::vector<float2> rb(kept);
-        CK(cudaMemcpy(ra.data(), dRA.p, 16 * kept, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), dRB.p, 8 * kept, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(ra.data(), t.dAdamRecA.p, 16 * kept, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), t.dAdamRecB.p, 8 * kept, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < kept; ++i) { memcpy(adam_records_out + 6 * i, &ra[i], 16); memcpy(adam_records_out + 6 * i + 4, &rb[i], 8); }
     }
     return PPG_OK;
@@ -1706,43 +1707,39 @@ extern "C" int ppg_op_adam_replay(int device, int loss, int bucket, float *state
     if (loss != PPG_LOSS_KL && loss != PPG_LOSS_VAR) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: loss is kl or var");
     if (!state_inout || !n_nodes || n_nodes >= 0xFFFFFFFFull || n_records >= 0xFFFFFFFFull || (n_records && !records) || (!bucket && (!leaf_offset || !leaf_count)))
         return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: empty or null input");
-    std::vector<float4> ra(std::max<size_t>(n_records, 1)); std::vector<float2> rb(std::max<size_t>(n_records, 1));
-    for (size_t i = 0; i < n_records; ++i) { memcpy(&ra[i], records + 6 * i, 16); memcpy(&rb[i], records + 6 * i + 4, 8); }
-    std::vector<float4> la(n_nodes);
-    for (size_t i = 0; i < n_nodes; ++i) la[i] = make_float4(0.f, 0.f, state_inout[6 * i + 3], 0.f);
-    const uint32_t sc0[8] = {(uint32_t) n_nodes, 0, 0, (uint32_t) n_records, 0, 0, 0, 0};
-    DevBuf<float4> dLA, dRA, dSA; DevBuf<float2> dRB, dSB; DevBuf<float> dAd; DevBuf<uint32_t> dCount, dCursor, dOff, dSc;
-    CK(dev_array(dLA, n_nodes, la.data(), n_nodes)); CK(dev_array(dAd, 6 * n_nodes, state_inout, 6 * n_nodes)); CK(dev_array(dSc, 8, sc0, 8));
-    CK(dev_array(dRA, n_records, ra.data(), n_records)); CK(dev_array(dRB, n_records, rb.data(), n_records));
-    MaintParams M; memset(&M, 0, sizeof(M));
-    M.leafA = dLA.p; M.adam = dAd.p; M.nNodes = dSc.p; M.capNodes = (uint32_t) n_nodes;
-    const int sms = op_sm_count();
-    if (bucket) {       // render_batch: histogram -> scan -> scatter into per-leaf buckets
-        CK(dev_array(dCount, n_nodes)); CK(dev_array(dCursor, n_nodes)); CK(dev_array(dOff, n_nodes)); CK(dev_array(dSA, n_records)); CK(dev_array(dSB, n_records));
-        adam_hist_kernel<<<sms * 4, 256>>>(dRA.p, dSc.p + 3, (uint32_t) n_records, dCount.p);
-        exclusive_scan_kernel<<<1, 1024>>>(dCount.p, dOff.p, dSc.p, dSc.p + 4);
-        adam_scatter_kernel<<<sms * 4, 256>>>(dRA.p, dRB.p, dSc.p + 3, (uint32_t) n_records, dOff.p, dCursor.p, dSA.p, dSB.p);
-        CK(cudaGetLastError());
-        if (bucketed_out && n_records) {
-            CK(cudaMemcpy(ra.data(), dSA.p, 16 * n_records, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), dSB.p, 8 * n_records, cudaMemcpyDeviceToHost));
-            for (size_t i = 0; i < n_records; ++i) { memcpy(bucketed_out + 6 * i, &ra[i], 16); memcpy(bucketed_out + 6 * i + 4, &rb[i], 8); }
-        }
-        if (leaf_offset_out) CK(cudaMemcpy(leaf_offset_out, dOff.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    } else {            // records already grouped; the cursors hold the counts, as after adam_scatter_kernel
+    if (!bucket)
         for (size_t i = 0; i < n_nodes; ++i)
             if ((size_t) leaf_offset[i] + leaf_count[i] > n_records) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: a leaf's records run past n_records");
-        CK(dev_array(dCount, n_nodes, leaf_count, n_nodes)); CK(dev_array(dCursor, n_nodes, leaf_count, n_nodes)); CK(dev_array(dOff, n_nodes, leaf_offset, n_nodes));
+    TreeStore t;
+    rc = t.load(0, n_nodes, (uint32_t) n_nodes, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, state_inout, 0, nullptr, nullptr); if (rc) return rc;
+    t.adamCap = n_records; CK(t.dAdamRecA.alloc(n_records)); CK(t.dAdamRecB.alloc(n_records)); CK(t.dAdamSortA.alloc(n_records)); CK(t.dAdamSortB.alloc(n_records));
+    std::vector<float4> ra(n_records); std::vector<float2> rb(n_records);
+    for (size_t i = 0; i < n_records; ++i) { memcpy(&ra[i], records + 6 * i, 16); memcpy(&rb[i], records + 6 * i + 4, 8); }
+    // records to bucket go where commit appends them; records already grouped go straight into the buckets
+    const uint32_t nRec = (uint32_t) n_records;
+    CK(cudaMemcpy(t.dScalars.p + 3, &nRec, 4, cudaMemcpyHostToDevice));
+    CK(t.put(bucket ? t.dAdamRecA : t.dAdamSortA, ra.data(), n_records));
+    CK(t.put(bucket ? t.dAdamRecB : t.dAdamSortB, rb.data(), n_records));
+    if (bucket) {
+        t.adam_bucket();
+        CK(cudaGetLastError());
+        if (bucketed_out && n_records) {
+            CK(cudaMemcpy(ra.data(), t.dAdamSortA.p, 16 * n_records, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), t.dAdamSortB.p, 8 * n_records, cudaMemcpyDeviceToHost));
+            for (size_t i = 0; i < n_records; ++i) { memcpy(bucketed_out + 6 * i, &ra[i], 16); memcpy(bucketed_out + 6 * i + 4, &rb[i], 8); }
+        }
+        if (leaf_offset_out) CK(cudaMemcpy(leaf_offset_out, t.dAdamOffset.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    } else {            // the cursors hold the counts, as after adam_scatter_kernel
+        CK(cudaMemcpy(t.dAdamCount.p, leaf_count, 4 * n_nodes, cudaMemcpyHostToDevice)); CK(cudaMemcpy(t.dAdamCursor.p, leaf_count, 4 * n_nodes, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(t.dAdamOffset.p, leaf_offset, 4 * n_nodes, cudaMemcpyHostToDevice));
         if (leaf_offset_out) memcpy(leaf_offset_out, leaf_offset, 4 * n_nodes);
     }
-    adam_seq_kernel<<<sms * 16, 128>>>(M, bucket ? dSA.p : dRA.p, bucket ? dSB.p : dRB.p, dOff.p, dCount.p, dCursor.p, loss == PPG_LOSS_KL ? 1.0f : 2.0f);
+    t.adam_replay(loss);
     CK(cudaGetLastError());
-    CK(cudaMemcpy(state_inout, dAd.p, 24 * n_nodes, cudaMemcpyDeviceToHost));
-    if (theta_out) {
-        CK(cudaMemcpy(la.data(), dLA.p, 16 * n_nodes, cudaMemcpyDeviceToHost));
-        for (size_t i = 0; i < n_nodes; ++i) theta_out[i] = la[i].z;
-    }
-    if (count_out) CK(cudaMemcpy(count_out, dCount.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
-    if (cursor_out) CK(cudaMemcpy(cursor_out, dCursor.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    TreeGather g; rc = t.gather(0, g); if (rc) return rc;
+    memcpy(state_inout, g.adam.data(), 24 * n_nodes);
+    if (theta_out) for (size_t i = 0; i < n_nodes; ++i) theta_out[i] = g.la[i].z;
+    if (count_out) CK(cudaMemcpy(count_out, t.dAdamCount.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    if (cursor_out) CK(cudaMemcpy(cursor_out, t.dAdamCursor.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
     return PPG_OK;
   });
 }
