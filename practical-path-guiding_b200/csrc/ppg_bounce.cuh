@@ -52,7 +52,8 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                 camera_ray(P, i, rng, sampleIndex, o, d, mint, maxt);
                 thr = f3(1, 1, 1); Li = f3(0, 0, 0);
             } else {
-                const float4 a = __ldcs(&P.in.s0[i]), b = __ldcs(&P.in.s1[i]), c = __ldcs(&P.in.s2[i]), e = __ldcs(&P.in.s3[i]), f = __ldcs(&P.in.s4[i]);   // streamed once: evict-first keeps the L2 for the trees
+                const uint32_t s = state_slot(i, (uint32_t) __ldg(P.splitIn), P.pathCapacity);     // reloaded (L1) rather than held across the loop
+                const float4 a = __ldcs(&P.in.s0[s]), b = __ldcs(&P.in.s1[s]), c = __ldcs(&P.in.s2[s]), e = __ldcs(&P.in.s3[s]), f = __ldcs(&P.in.s4[s]);   // streamed once: evict-first keeps the L2 for the trees
                 o = f3(a.x, a.y, a.z); d = f3(a.w, b.x, b.y); thr = f3(b.z, b.w, c.x); eta = c.y; Li = f3(c.z, c.w, e.x);
                 pathId = __float_as_uint(e.y);
                 rng.state = ((uint64_t) __float_as_uint(e.w) << 32) | __float_as_uint(e.z);
@@ -60,12 +61,12 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                 rng.inc = (sampleIndex << 1) | 1u;
                 const uint32_t nf = __float_as_uint(f.z); nVertices = nf & 0xffu; flags = nf >> 8;
                 rrRecip = f.w;
-                if (NEE) { const float4 g5 = __ldcs(&P.in.s5[i]), g6 = __ldcs(&P.in.s6[i]); prevWoPdf = g5.x; prevRefN = f3(g5.y, g5.z, g5.w); prevSlot = __float_as_uint(g6.x); }
+                if (NEE) { const float4 g5 = __ldcs(&P.in.s5[s]), g6 = __ldcs(&P.in.s6[s]); prevWoPdf = g5.x; prevRefN = f3(g5.y, g5.z, g5.w); prevSlot = __float_as_uint(g6.x); }
                 mint = surface_ray_mint(o);
                 maxt = __int_as_float(0x7f800000);
             }
         }
-        bool wroteVertex = false, wroteNee = false, unscattered = FIRST;
+        bool wroteVertex = false, wroteNee = false, unscattered = FIRST, dtreeNext = false;
         Hit hit; bool rayOk = false, found = false;
         if (alive) {
             ++raysLocal;
@@ -248,6 +249,16 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
                         }
                     }
                 }
+                if (P.isBuilt && !binned) {
+                    // the next vertex's technique (its sampleMat: sx = the draw after this vertex's Russian roulette, D-tree when sx >= frac),
+                    // predicted here where frac is last needed -- exact for a fixed fraction; with a learned one the next leaf's fraction
+                    // decides, and a wrong guess only costs divergence.  It places the path in the output wavefront (warp_compact_split) and
+                    // changes nothing the path computes.  Material-binned launches take their warps from the bins instead: there the split
+                    // would only spread the rays of a trace_kernel warp over twice the pixels (TORUS: 3.6 % slower), so every path stays in front.
+                    Pcg32 peek = rng;
+                    if (!(FULL && isNull) && P.depth >= P.rrDepth) peek.nextU32();
+                    dtreeNext = !(peek.next1D() < frac);
+                }
                 if (is_zero(bsdfWeight)) cont = false;                               // GP:2024-2025
                 float3 woW = f3(0, 0, 0);
                 if (cont) {
@@ -293,7 +304,7 @@ __global__ void __launch_bounds__(SMEM ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM
         }
         if (RECORD && i < nIn && !wroteVertex) __stcs(&P.slab.v2[i], make_float4(0.f, 0.f, 0.f, __uint_as_float(PPG_INVALID)));
         if (NEE && RECORD && P.neeMode != 2 && i < nIn && !wroteNee) __stcs(&P.neeSlab.v2[i], make_float4(0.f, 0.f, 0.f, __uint_as_float(PPG_INVALID)));
-        const uint32_t slot = warp_compact(alive, P.liveOut);
+        const uint32_t slot = warp_compact_split(alive, dtreeNext, P.splitOut, P.liveOut, P.pathCapacity);
         if (alive) {
             __stcs(&P.out.s0[slot], make_float4(o.x, o.y, o.z, d.x));
             __stcs(&P.out.s1[slot], make_float4(d.y, d.z, thr.x, thr.y));

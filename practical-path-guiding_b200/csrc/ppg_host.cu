@@ -452,7 +452,7 @@ struct ppg_integrator {
 
     // wavefront
     size_t pathCapacity = 0; int maxBounces = 0, nSlabs = 0; int recordMode = 0; int stateVecs = 5, slabSets = 1;
-    DevBuf<float4> dStateA, dStateB, dSlabs, dLiFinal; DevBuf<uint32_t> dLive, dWork; DevBuf<unsigned long long> dCounters;
+    DevBuf<float4> dStateA, dStateB, dSlabs, dLiFinal; DevBuf<uint32_t> dLive, dWork; DevBuf<unsigned long long> dSplit, dCounters;
     DevBuf<float4> dHits; DevBuf<uint32_t> dTraceWork; int gridTrace = 0; uint32_t traceMinPaths = 0;   // separate nearest-hit pass (ppg_trace.cu), BVH scenes only
     DevBuf<uint32_t> dOrder, dBinCount; bool binMaterials = false;                                        // ... which also bins the paths by the BSDF class they hit
     int gridBounce = 0;
@@ -826,7 +826,7 @@ static int ensure_wavefront(ppg_integrator *h) {
         CK(h->dSlabs.alloc((size_t) h->nSlabs * (full ? 6 : 3) * cap * slabSets));
         h->pathCapacity = cap; h->stateVecs = stateVecs; h->slabSets = slabSets;
     }
-    CK(h->dLive.alloc(h->maxBounces + 2)); CK(h->dWork.alloc(h->maxBounces + 2)); CK(h->dCounters.alloc(8));
+    CK(h->dLive.alloc(h->maxBounces + 2)); CK(h->dSplit.alloc(h->maxBounces + 2)); CK(h->dWork.alloc(h->maxBounces + 2)); CK(h->dCounters.alloc(8));
     if (h->prm.bsdf_sampling_fraction_loss != PPG_LOSS_NONE) {
         // sampling-fraction records: one per (recorded vertex, leaf) pair.  Sized once for the largest wavefront with 16 records per path (mean path
         // lengths of the bundled scenes: 4 - 9 vertices; the spatial box filter touches ~2 leaves per vertex); a record beyond it is dropped and
@@ -895,9 +895,11 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
     if (nPaths) {
         CK(cudaMemsetAsync(h->dLive.p, 0, 4 * (size_t) (h->maxBounces + 2), h->stream));
         CK(cudaMemsetAsync(h->dWork.p, 0, 4 * (size_t) (h->maxBounces + 2), h->stream));
+        CK(cudaMemsetAsync(h->dSplit.p, 0, 8 * (size_t) (h->maxBounces + 2), h->stream));
         CK(cudaMemcpyAsync(h->dLive.p, &nPaths, 4, cudaMemcpyHostToDevice, h->stream));
         RenderParams P;
         P.scene = h->sceneView; P.cam = h->cam; P.tree = h->tree.view(h->aabbMin, h->extent);
+        P.pathCapacity = (uint32_t) h->pathCapacity;
         P.liFinal = h->dLiFinal.p; P.pixelMap = pixelMap; P.counters = h->dCounters.p;
         P.nPaths = nPaths; P.nLocalPixels = pixelCount; P.spp = (uint32_t) h->prm.spp_per_pass;
         P.passBase = (uint64_t) h->passesRendered; P.seed = h->prm.seed;
@@ -918,6 +920,7 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
         for (int depth = 1; depth <= h->maxBounces; ++depth) {
             P.depth = depth; P.in = (depth & 1) ? B : A; P.out = (depth & 1) ? A : B;
             P.liveIn = h->dLive.p + (depth - 1); P.liveOut = h->dLive.p + depth; P.work = h->dWork.p + depth;
+            P.splitIn = h->dSplit.p + (depth - 1); P.splitOut = h->dSplit.p + depth;
             const int k = std::min(depth - 1, h->nSlabs - 1);
             P.slab = slab_at(h, k);
             if (nee) { P.neeSlab = slab_at(h, k, 1); P.prevSlab = slab_at(h, std::max(k - 1, 0)); if (depth - 1 >= h->nSlabs) P.prevSlab = slab_at(h, h->nSlabs - 1); }
@@ -950,7 +953,7 @@ static int render_batch(ppg_integrator *h, int nPasses, const uint32_t *pixelMap
         if (bracket) h->toc(bracket);
         {   // survivors of the bounce cap (maxDepth == -1 only) keep the radiance they have; they are counted (ppg_stats.truncated_paths)
             const PathState last = (lastDepth & 1) ? A : B;
-            flush_kernel<<<std::max(grid / 4, 1), PPG_BLOCK, 0, h->stream>>>(last, h->dLive.p + lastDepth, h->dLiFinal.p, h->dCounters.p + 3); h->launches++;
+            flush_kernel<<<std::max(grid / 4, 1), PPG_BLOCK, 0, h->stream>>>(last, h->dLive.p + lastDepth, h->dSplit.p + lastDepth, (uint32_t) h->pathCapacity, h->dLiFinal.p, h->dCounters.p + 3); h->launches++;
         }
         if (record) {
             CommitParams C;

@@ -6,11 +6,12 @@
 namespace ppg {
 
 // paths still alive after the last bounce (only possible with maxDepth == -1 and the bounce cap) keep their radiance; counted in *truncated
-__global__ void __launch_bounds__(PPG_BLOCK) flush_kernel(PathState in, const uint32_t *liveIn, float4 *liFinal, unsigned long long *truncated) {
-    const uint32_t nIn = *liveIn;
+__global__ void __launch_bounds__(PPG_BLOCK) flush_kernel(PathState in, const uint32_t *liveIn, const unsigned long long *splitIn, uint32_t cap, float4 *liFinal, unsigned long long *truncated) {
+    const uint32_t nIn = *liveIn; const uint32_t nFront = (uint32_t) *splitIn;
     if (blockIdx.x == 0 && threadIdx.x == 0 && nIn) atomicAdd(truncated, (unsigned long long) nIn);
     for (uint32_t i = blockIdx.x * PPG_BLOCK + threadIdx.x; i < nIn; i += gridDim.x * PPG_BLOCK) {
-        const float4 c = in.s2[i], e = in.s3[i];
+        const uint32_t s = state_slot(i, nFront, cap);
+        const float4 c = in.s2[s], e = in.s3[s];
         liFinal[__float_as_uint(e.y)] = make_float4(c.z, c.w, e.x, 1.f);
     }
 }

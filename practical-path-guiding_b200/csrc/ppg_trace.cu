@@ -33,6 +33,7 @@ __global__ void __launch_bounds__(PPG_TRACE_BLOCK, PPG_TRACE_MIN_BLOCKS) trace_k
     const SceneAccess<false> A_(P.scene);
     const SceneView &sc = P.scene;
     const uint32_t nIn = FIRST ? P.nPaths : *P.liveIn;
+    const uint32_t nFront = FIRST ? 0u : (uint32_t) *P.splitIn;
     const uint32_t lane = threadIdx.x & 31u, lt = (1u << lane) - 1u;
     bool active = false, done = false, exhausted = false;
     uint32_t my = 0, left = 0, count = 0;
@@ -60,7 +61,8 @@ __global__ void __launch_bounds__(PPG_TRACE_BLOCK, PPG_TRACE_MIN_BLOCKS) trace_k
                 my = take;
                 if (FIRST) { Pcg32 rng; uint64_t sampleIndex; camera_ray(P, my, rng, sampleIndex, o, d, mint, maxt); }
                 else {
-                    const float4 a = P.in.s0[my], b = P.in.s1[my];
+                    const uint32_t s = state_slot(my, nFront, P.pathCapacity);       // hits and bins are indexed by `my`, the compact index
+                    const float4 a = P.in.s0[s], b = P.in.s1[s];
                     o = f3(a.x, a.y, a.z); d = f3(a.w, b.x, b.y);
                     mint = surface_ray_mint(o); maxt = __int_as_float(0x7f800000);
                 }

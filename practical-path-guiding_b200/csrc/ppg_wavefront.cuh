@@ -5,7 +5,7 @@
 //     bounce         (one launch per further path depth)  GP:1798-2146
 //     commit         (all recorded vertices -> building trees)   GP:2150-2154 -> 1730-1768 -> 575-584
 //     film           (per-pixel sum and sum of squares)   GP:1633-1634, imageblock.h:127-186
-// Live paths are compacted between bounces (warp ballot + prefix popcount + one atomic per warp),
+// Live paths are compacted between bounces (warp ballot + prefix popcount + one atomic per warp, ordered by the next vertex's sampling technique),
 // path state is SoA float4 (5 x 16 B per path, coalesced), the scene (CBOX: ~9 KB) is staged in
 // shared memory, the read-only sampling trees go through the read-only/L1 path.
 #pragma once
@@ -65,6 +65,10 @@ struct RenderParams {
     float4 *liFinal;               // per path: Li.rgb, 1
     const uint32_t *pixelMap;      // local pixel -> x | y<<16
     const uint32_t *liveIn; uint32_t *liveOut;      // device counters
+    // Survivors are stored by the sampling technique their next vertex is predicted to take (see warp_compact_split): nFront | nBack << 32
+    // of the input / output wavefront.  The input's compact index j lives at state_slot(j, nFront, pathCapacity).
+    const unsigned long long *splitIn; unsigned long long *splitOut;
+    uint32_t pathCapacity;                          // entries of each PathState array
     uint32_t *work;                                 // dynamic scheduling: next unclaimed input index of this launch (zeroed by the host), or nullptr
     unsigned long long *counters;  // [0]: rays traced, [1]: vertices recorded, [2]: sum of S-tree levels over recorded vertices, [3]: truncated paths,
                                    // [4]: dropped sampling-fraction records, [5]: rays with a non-finite origin / direction
@@ -116,15 +120,29 @@ __device__ __forceinline__ void camera_ray(const RenderParams &P, uint32_t i, Pc
 // adaptive ray epsilon of rays leaving a surface (skdtree.cpp:125-128)
 __device__ __forceinline__ float surface_ray_mint(float3 o) { return PPG_EPSILON * fmaxf(fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fabsf(o.z)), PPG_EPSILON); }
 
-// warp-wide compaction: returns the output slot of this lane (valid when `alive`); one atomic per warp and
-// no block barrier, so warps of a block never wait for each other inside the path loop.
-__device__ __forceinline__ uint32_t warp_compact(bool alive, uint32_t *counter) {
-    const unsigned ballot = __ballot_sync(0xffffffffu, alive);
+// warp-wide compaction: returns the output slot of this lane (valid when `alive`); no block barrier, so warps of a block never wait for
+// each other inside the path loop.  The survivors are split by `back` (the next vertex is predicted to sample the D-tree): front paths fill
+// the PathState from slot 0 upward, back paths from slot cap - 1 downward, so that a guided warp of the next bounce holds lanes of one
+// technique and issues one branch of sampleMat (only the warp that straddles the boundary holds both).  One returning 64-bit atomic per
+// warp on split = nFront | nBack << 32 claims both ranges; the total (liveOut: commit's slab counts, the host's read-back) is added
+// without waiting for its result.
+__device__ __forceinline__ uint32_t warp_compact_split(bool alive, bool back, unsigned long long *split, uint32_t *total, uint32_t cap) {
+    const unsigned live = __ballot_sync(0xffffffffu, alive), backs = __ballot_sync(0xffffffffu, alive && back);
     const int lane = threadIdx.x & 31;
-    uint32_t base = 0;
-    if (lane == 0 && ballot) base = atomicAdd(counter, (uint32_t) __popc(ballot));
+    unsigned long long base = 0;
+    if (lane == 0 && live) {
+        const uint32_t nAlive = __popc(live), nBack = __popc(backs);
+        base = atomicAdd(split, (unsigned long long) (nAlive - nBack) | ((unsigned long long) nBack << 32));
+        atomicAdd(total, nAlive);
+    }
     base = __shfl_sync(0xffffffffu, base, 0);
-    return base + __popc(ballot & ((1u << lane) - 1u));
+    const unsigned below = (1u << lane) - 1u;
+    return back ? cap - 1u - ((uint32_t) (base >> 32) + __popc(backs & below)) : (uint32_t) base + __popc(live & ~backs & below);
+}
+// PathState slot of compact index j of a wavefront written by warp_compact_split (nFront: the low half of its split counter): compact indices
+// enumerate the front range, then the back range from its first-written slot.  Slabs, hit records and material bins keep using j.
+__device__ __forceinline__ uint32_t state_slot(uint32_t j, uint32_t nFront, uint32_t cap) {
+    return j < nFront ? j : cap - 1u - (j - nFront);
 }
 
 // The bounce kernel itself lives in ppg_bounce.cuh; it is compiled in four translation units (ppg_bounce_inst.cu with
