@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define PPG_ABI_VERSION 2   /* 2: bitmap textures, bumpmap, environment map */
+#define PPG_ABI_VERSION 3   /* 2: bitmap textures, bumpmap, environment map; 3: SD-trees cross as one ppg_sdtree */
 
 typedef enum ppg_status {
     PPG_OK = 0,
@@ -368,18 +368,35 @@ int ppg_cancel(ppg_integrator *h);
 /* dumpSDTree wire format (GP:1191-1208, 699-711, 945-951), current sampling trees. */
 int ppg_dump_sdtree(ppg_integrator *h, const char *path);
 
-/* The integrator's SD-tree as flat host arrays, after ppg_render or from inside the film callback (after an iteration's passes, before its
- * build: the S-tree is refined, the sampling trees are the ones the passes guided with, the building trees hold what they recorded).
- * which: 0 = sampling trees, 1 = building trees.  Per S-tree node, in the integrator's own numbering: node_children (2 x u32, 0 0 for a leaf),
- * tree_first (u64 offset of the node's quadtree in sums / children), tree_count, tree_depth, tree_sum, tree_weight (sampling: the tree's sum and
- * statistical weight; building: sum 0 and the weight recorded so far), adam (6 floats: iter, m, v, theta as the bounce kernel reads it,
- * batchAcc, batchGrad).  Inner nodes carry zeros.  The quadtrees of the leaves, concatenated in node order: sums (4 floats) and children
- * (4 x u16) per quadtree node.  aabb_min_max: the cubified S-tree box (6 floats).  Output arrays hold node_capacity nodes and pool_capacity
- * quadtree nodes; if either is too small the call returns PPG_ERR_INVALID_ARGUMENT with *n_nodes_out and *n_pool_out set to the sizes
- * needed.  Output pointers other than the counts may be NULL. */
-int ppg_export_sdtree(ppg_integrator *h, int which, size_t node_capacity, size_t *n_nodes_out, uint32_t *node_children, uint64_t *tree_first,
-                      uint32_t *tree_count, int32_t *tree_depth, float *tree_sum, float *tree_weight, float *adam,
-                      size_t pool_capacity, size_t *n_pool_out, float *sums, uint16_t *children, float *aabb_min_max);
+/* An SD-tree as flat host arrays: the S-tree and, per leaf, one quadtree (a D-tree) -- the sampling trees or the building trees.
+ * Per S-tree node, in the integrator's own numbering:
+ *   node_children  2 x u32: child 0, child 1 (0 0: a leaf; the split axis cycles x, y, z from the root)
+ *   tree_first     u64 offset of the node's quadtree in sums / children (below 2^32 on input)
+ *   tree_count     quadtree nodes, tree_depth m_maxDepth, tree_sum / tree_weight DTree::m_atomic (GP:538-557)
+ *   adam           6 floats: iter, m, v, theta as the bounce kernel reads it, batchAcc, batchGrad (GP:69-133)
+ * Per quadtree node, the leaves' quadtrees concatenated: sums (4 floats) and children (4 x u16, 0 = leaf), the reference's QuadTreeNode
+ * (GP:158-371, 368-370).
+ * A building tree has tree_sum 0 and its tree_weight is the statistical weight recorded so far.  Inner nodes carry no tree: zero count,
+ * depth, sum, weight and Adam state.
+ * On input a NULL array stands for zeros, and n_nodes / n_pool give the lengths.  On output a NULL array is not wanted; the arrays hold
+ * node_capacity nodes and pool_capacity quadtree nodes, n_nodes / n_pool receive the sizes, and if either capacity is too small the call
+ * returns PPG_ERR_INVALID_ARGUMENT with the sizes set. */
+typedef struct ppg_sdtree {
+    size_t    n_nodes, node_capacity;
+    uint32_t *node_children;
+    uint64_t *tree_first;
+    uint32_t *tree_count;
+    int32_t  *tree_depth;
+    float    *tree_sum, *tree_weight, *adam;
+    size_t    n_pool, pool_capacity;
+    float    *sums;
+    uint16_t *children;
+} ppg_sdtree;
+
+/* The integrator's SD-tree, after ppg_render or from inside the film callback (after an iteration's passes, before its build: the S-tree
+ * is refined, the sampling trees are the ones the passes guided with, the building trees hold what they recorded).  which: 0 = sampling
+ * trees, 1 = building trees.  aabb_min_max (or NULL): the cubified S-tree box (6 floats). */
+int ppg_export_sdtree(ppg_integrator *h, int which, ppg_sdtree *out, float *aabb_min_max);
 
 /* scene->getDestinationFile(): with dumpSDTree=true every non-final iteration writes "<destination>-NN.sdt"
  * (NN = two-digit iteration index, GP:1191-1195, 1417-1419). NULL/"" disables the per-iteration dumps. */
@@ -397,34 +414,22 @@ const char *ppg_last_error(void);
 
 /* ---- batch operators on SD-tree arrays (kernel-level entry points) ------------------- *
  * These run the SAME device functions the render kernels use on caller-supplied
- * flat tree arrays, so parity tests can compare them element-wise against the
- * oracle. All pointers are HOST pointers; copies happen inside.
- *
- * D-tree arrays: node i has sums[4*i..4*i+3] and children[4*i..4*i+3]
- * (uint16, 0 = leaf), the reference's QuadTreeNode (GP:158-371, 368-370).
- * tree_first_node[t] is the index of the root of tree t; tree_sum / tree_weight
- * are DTree::m_atomic (GP:538-557).                                                    */
+ * trees, so parity tests can compare them element-wise against the oracle.
+ * All pointers are HOST pointers; copies happen inside.  The D-tree queries take a
+ * tree without node_children: every node is then a leaf, and a query names its node. */
 
-/* DTreeWrapper::pdf (GP:623-625 -> 415-421, 232-245): n directions (xyz). */
-int ppg_op_dtree_pdf(int device,
-                     const float *sums, const uint16_t *children, size_t n_nodes,
-                     const uint32_t *tree_first_node, const float *tree_sum, const float *tree_weight, size_t n_trees,
-                     const uint32_t *query_tree, const float *query_dir, size_t n, float *pdf_out);
+/* DTreeWrapper::pdf (GP:623-625 -> 415-421, 232-245) in the sampling trees: n directions (xyz). */
+int ppg_op_dtree_pdf(int device, const ppg_sdtree *tree, const uint32_t *query_tree, const float *query_dir, size_t n, float *pdf_out);
 
-/* DTreeWrapper::sample (GP:619-621 -> 431-442, 257-301) with REPLAYED uniforms:
+/* DTreeWrapper::sample (GP:619-621 -> 431-442, 257-301) in the sampling trees with REPLAYED uniforms:
  * rnd holds rnd_stride floats per query, consumed in the reference's order (one per level, two at the leaf).
  * dir_out: 3 floats per query.  canonical_out (2 floats per query, or NULL): the point DTree::sample returns, before canonicalToDir. */
-int ppg_op_dtree_sample(int device,
-                        const float *sums, const uint16_t *children, size_t n_nodes,
-                        const uint32_t *tree_first_node, const float *tree_sum, const float *tree_weight, size_t n_trees,
-                        const uint32_t *query_tree, const float *rnd, size_t rnd_stride, size_t n, float *dir_out, float *canonical_out);
+int ppg_op_dtree_sample(int device, const ppg_sdtree *tree, const uint32_t *query_tree, const float *rnd, size_t rnd_stride, size_t n,
+                        float *dir_out, float *canonical_out);
 
-/* DTreeWrapper::record (GP:575-584 -> 395-413, 303-338) for n records into the
- * building sums (in/out) and per-tree statistical weights (in/out); filter = ppg_directional_filter. */
-int ppg_op_dtree_record(int device,
-                        float *sums_inout, const uint16_t *children, size_t n_nodes,
-                        const uint32_t *tree_first_node, float *tree_weight_inout, size_t n_trees,
-                        const uint32_t *rec_tree, const float *rec_dir, const float *rec_radiance,
+/* DTreeWrapper::record (GP:575-584 -> 395-413, 303-338) of n records into the building trees: their sums and tree_weight are
+ * updated in place.  filter = ppg_directional_filter. */
+int ppg_op_dtree_record(int device, const ppg_sdtree *tree, const uint32_t *rec_tree, const float *rec_dir, const float *rec_radiance,
                         const float *rec_wo_pdf, const float *rec_weight, size_t n, int filter);
 
 /* The acceleration structure ppg_set_scene builds over the scene's triangles (binned-SAH BVH; it takes the place of the reference's ShapeKDTree,
@@ -448,51 +453,36 @@ int ppg_op_emitter_sample_direct(ppg_integrator *h, size_t n, const float *ref, 
  * discrete emitter choice) for n world directions d (3n), and optionally its radiance there (evalEnvironment, :380-410; value_out 3n or NULL). */
 int ppg_op_env_pdf(ppg_integrator *h, size_t n, const float *d, float *pdf_out, float *value_out);
 
-/* STree::dTreeWrapper(p, size) (GP:897-905, 761-769): S-tree nodes as uint32
- * pairs (child0, child1); child0 == 0 marks a leaf. Outputs the leaf NODE index
- * and the voxel size (3 floats) per query point. */
-int ppg_op_stree_lookup(int device,
-                        const uint32_t *node_children, size_t n_nodes,
-                        const float aabb_min[3], const float aabb_extent[3],
+/* STree::dTreeWrapper(p, size) (GP:897-905, 761-769) in the S-tree of `tree` (its node_children): the leaf NODE index and the voxel
+ * size (3 floats) per query point. */
+int ppg_op_stree_lookup(int device, const ppg_sdtree *tree, const float aabb_min[3], const float aabb_extent[3],
                         const float *points, size_t n, uint32_t *leaf_out, float *size_out);
 
 /* ---- the learning half: the render's own maintenance, commit and Adam kernels on caller-supplied trees ----------------- *
- * S-tree arrays per node: node_children (2 uint32, child0 == 0: leaf; the split axis cycles x, y, z from the root), and per leaf its
- * sampling tree (tree_first = root in the sampling pool, tree_count nodes, tree_depth = m_maxDepth, tree_sum / tree_weight = m_atomic),
- * its building weight and adam = 6 floats {iter, m1, m2, theta, batchAcc, batchGrad} (GP:69-133).  Pools as above. */
+ * The trees these ops hand back keep the input's quadtree offsets: tree_first indexes the pool as the device holds it, which the ops load
+ * at the caller's offsets, and n_pool is where the last leaf's quadtree ends. */
 
-/* resetSDTree (GP:1108-1113): stages bit 0 = STree::refine (GP:957-998; split while the building weight exceeds `threshold`),
- * bit 1 = DTree::reset of every leaf (GP:456-514) with new_max_depth and dtree_threshold.  node_capacity 0: sized as the render sizes it;
- * a refinement that runs out of it returns PPG_ERR_CUDA.  Outputs: the S-tree after the refine with the inherited per-node fields
- * (building_weight_out: after the refine, before the reset clears it) and, per leaf, the new building tree (build_first/count/depth into
- * build_children_out / build_sums_out).  Output arrays hold out_capacity nodes and build_capacity pool nodes; if either is too small the call
- * returns PPG_ERR_INVALID_ARGUMENT with *n_nodes_out and *n_build_out set to the sizes needed.  Output pointers other than the counts may be NULL. */
+/* resetSDTree (GP:1108-1113) on the sampling tree `in` and per-node building_weight: stages bit 0 = STree::refine (GP:957-998; split while
+ * the building weight exceeds `threshold`), bit 1 = DTree::reset of every leaf (GP:456-514) with new_max_depth and dtree_threshold.
+ * node_capacity 0: sized as the render sizes it; a refinement that runs out of it returns PPG_ERR_CUDA.  Outputs: the refined S-tree's
+ * sampling trees (a new leaf shares its parent's quadtree in the input pool) and the new building trees, whose tree_weight is the building
+ * weight after the refine, before the reset clears it. */
 int ppg_op_sdtree_refine_reset(int device, int stages, float threshold, int new_max_depth, float dtree_threshold, size_t node_capacity,
-                               const uint32_t *node_children, size_t n_nodes, const uint32_t *tree_first, const uint32_t *tree_count, const int32_t *tree_depth,
-                               const float *tree_sum, const float *tree_weight, const float *adam, const float *building_weight,
-                               const float *sums, const uint16_t *children, size_t n_pool,
-                               size_t out_capacity, size_t *n_nodes_out, uint32_t *node_children_out, uint32_t *tree_first_out, uint32_t *tree_count_out,
-                               int32_t *tree_depth_out, float *tree_sum_out, float *tree_weight_out, float *adam_out, float *building_weight_out,
-                               uint32_t *build_first_out, uint32_t *build_count_out, int32_t *build_depth_out,
-                               size_t build_capacity, size_t *n_build_out, uint16_t *build_children_out, float *build_sums_out);
+                               const ppg_sdtree *in, const float *building_weight, ppg_sdtree *sampling_out, ppg_sdtree *building_out);
 
-/* buildSDTree (GP:1115-1189): DTree::build of every leaf's building tree (build_first/count/depth, building_weight, pool sums/children) and
- * "sampling = building".  Outputs: the sampling pool (same indices as the building pool), per node m_atomic sum / weight, depth, node count,
- * mean() > 0, and stats_out = 14 doubles {leaves, leaves with nodes, depth min, depth max, mean min, mean max, weight min, weight max,
- * nodes min, nodes max, depth sum, mean sum, nodes sum, weight sum} (the "distribution statistics", GP:1121-1186). */
-int ppg_op_sdtree_build(int device, const uint32_t *node_children, size_t n_nodes, const uint32_t *build_first, const uint32_t *build_count,
-                        const int32_t *build_depth, const float *building_weight, const float *sums, const uint16_t *children, size_t n_pool,
-                        float *sampling_sums_out, uint16_t *sampling_children_out, float *tree_sum_out, float *tree_weight_out,
-                        int32_t *tree_depth_out, uint32_t *tree_count_out, uint8_t *mean_positive_out, double *stats_out);
+/* buildSDTree (GP:1115-1189): DTree::build of every leaf's building tree and "sampling = building".  Outputs: the sampling trees (at the
+ * building trees' offsets), per node mean() > 0 (mean_positive_out, or NULL) and stats_out (or NULL) = 14 doubles {leaves, leaves with
+ * nodes, depth min, depth max, mean min, mean max, weight min, weight max, nodes min, nodes max, depth sum, mean sum, nodes sum, weight sum}
+ * (the "distribution statistics", GP:1121-1186). */
+int ppg_op_sdtree_build(int device, const ppg_sdtree *building, ppg_sdtree *sampling_out, uint8_t *mean_positive_out, double *stats_out);
 
-/* Vertex::commit (GP:1730-1768) of n path vertices through the render's commit kernel (record_mode 1: three vertex fields, nearest only;
- * 2: six).  vertices: 24 floats per vertex, the six float4 the bounce kernel writes {d, woPdf}, {throughput, bits(leaf)},
- * {radiance prefix, bits(path | absolute << 30 | delta << 31)}, {bsdf value, bsdfPdf}, {o, dTreePdf}, {bits(sampleIndex lo), bits(hi),
- * bits(S-tree levels | ordinal << 8), 0}; li_final: 4 floats per path.  Building weights and sums are updated in place.  With a loss the
+/* Vertex::commit (GP:1730-1768) of n path vertices into the building trees (sums and tree_weight updated in place) through the render's
+ * commit kernel (record_mode 1: three vertex fields, nearest only; 2: six).  vertices: 24 floats per vertex, the six float4 the bounce
+ * kernel writes {d, woPdf}, {throughput, bits(leaf)}, {radiance prefix, bits(path | absolute << 30 | delta << 31)}, {bsdf value, bsdfPdf},
+ * {o, dTreePdf}, {bits(sampleIndex lo), bits(hi), bits(S-tree levels | ordinal << 8), 0}; li_final: 4 floats per path.  With a loss the
  * sampling-fraction records are appended to adam_records_out (6 floats: bits(leaf), product, woPdf, bsdfPdf, dTreePdf, weight; up to
  * adam_capacity), *n_adam_out = records produced. */
-int ppg_op_commit(int device, int record_mode, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
-                  const uint32_t *build_first, float *building_weight_inout, float *sums_inout, const uint16_t *children, size_t n_pool,
+int ppg_op_commit(int device, int record_mode, const ppg_sdtree *building, const float aabb_min[3], const float aabb_extent[3],
                   const float *vertices, size_t n, const float *li_final, size_t n_li, int spatial_filter, int directional_filter, int loss,
                   uint64_t seed, float statistical_weight, float *adam_records_out, size_t adam_capacity, size_t *n_adam_out);
 

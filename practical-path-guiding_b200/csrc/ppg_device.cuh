@@ -1037,6 +1037,13 @@ struct TreeView {
     float3 aabbMin, extent;       // cubified scene box (GP:850-860)
 };
 
+// DTree::mean() (GP:387-393) of a tree whose m_atomic holds `sum` and statistical weight `weight`; mean > 0 is the flag bit of leafA
+__host__ __device__ __forceinline__ float dtree_mean(float sum, float weight) {
+    float mean = 0.f;
+    if (weight != 0.f) { const float factor = 1.f / (PPG_PI * 4.f * weight); mean = factor * sum; }
+    return mean;
+}
+
 __device__ __forceinline__ uint32_t child16(uint2 c, int i) { return ((i & 2) ? c.y : c.x) >> ((i & 1) * 16) & 0xffffu; }
 __device__ __forceinline__ float sum4(float4 s, int i) { return i == 0 ? s.x : (i == 1 ? s.y : (i == 2 ? s.z : s.w)); }
 

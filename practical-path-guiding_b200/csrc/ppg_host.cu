@@ -207,25 +207,26 @@ extern "C" void ppg_scene_file_free(ppg_scene_file *file) { delete file; }
 // ------------------------------------------------------------------ SD-tree storage and its launch sequences
 static float bits_f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 static uint32_t f_bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+// the ABI's quadtree nodes (NULL: zeros) as sampling-pool nodes: children keep their bytes, uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
 static std::vector<SampNode> to_pool(const float *sums, const uint16_t *children, size_t n) {
     std::vector<SampNode> pool(n);
     for (size_t i = 0; i < n; ++i) {
-        pool[i].sums = make_float4(sums[4 * i], sums[4 * i + 1], sums[4 * i + 2], sums[4 * i + 3]);
-        pool[i].children = make_uint2((uint32_t) children[4 * i] | ((uint32_t) children[4 * i + 1] << 16), (uint32_t) children[4 * i + 2] | ((uint32_t) children[4 * i + 3] << 16));
-        pool[i].pad = make_uint2(0u, 0u);
+        if (sums) memcpy(&pool[i].sums, sums + 4 * i, 16);
+        if (children) memcpy(&pool[i].children, children + 4 * i, 8);
     }
     return pool;
 }
-
-// An SD-tree on the host: the S-tree and, per node, either the sampling trees (which == 0: the trees the passes guide with) or the
-// building trees (which == 1: the trees the passes record into).  Between the reset and the build of an iteration (the film callback) the sampling
-// trees still sit where the previous build put them, past the new building total: the copy of the quadtree pool is sized from the leaves (or `minPool`).
-struct TreeGather {
-    uint32_t n = 0;
-    std::vector<uint2> sn; std::vector<float4> la; std::vector<float> sum, weight, adam; std::vector<int> depth; std::vector<uint32_t> count;
-    std::vector<uint2> children; std::vector<float4> sums;      // the quadtree pool from offset 0 (building: bchildren / bsums; sampling: dSamp)
-    uint32_t first(uint32_t i, int which) const { uint32_t u; memcpy(&u, which ? &la[i].y : &la[i].x, 4); return u; }
-};
+// the 6-float sampling-fraction record of the ABI <-> the float4 + float2 pair the device keeps it in
+static void records_split(const float *r, size_t n, std::vector<float4> &a, std::vector<float2> &b) {
+    a.resize(n); b.resize(n);
+    for (size_t i = 0; i < n; ++i) { memcpy(&a[i], r + 6 * i, 16); memcpy(&b[i], r + 6 * i + 4, 8); }
+}
+static int records_join(const float4 *dA, const float2 *dB, size_t n, float *r) {
+    std::vector<float4> a(n); std::vector<float2> b(n);
+    CK(cudaMemcpy(a.data(), dA, 16 * n, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(b.data(), dB, 8 * n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; ++i) { memcpy(r + 6 * i, &a[i], 16); memcpy(r + 6 * i + 4, &b[i], 8); }
+    return PPG_OK;
+}
 
 // The SD-tree on the device and its launch sequences, shared by the render and the ppg_op_* entry points.  Launch members return their launch count.
 struct TreeStore {
@@ -303,25 +304,27 @@ struct TreeStore {
         return PPG_OK;
     }
 
-    // The flat arrays of the ppg_op_* entry points (null: zeros) on the default stream, in exactly `nodeCap` S-tree and `nPool` quadtree nodes;
-    // first / count / depth / weight and the pool are the sampling trees (which == 0) or the building trees (which == 1)
-    int load(int which, size_t n, uint32_t nodeCap, const uint32_t *nodeChildren, const uint32_t *first, const uint32_t *count, const int32_t *depth,
-             const float *sum, const float *weight, const float *adam, size_t nPool, const float *sums, const uint16_t *children) {
+    // A caller's ppg_sdtree on the default stream, in exactly max(nodeCap, n_nodes) S-tree and n_pool quadtree nodes: the sampling trees
+    // (which == 0), with the leafA flag dtree_build_kernel writes, or the building trees (which == 1)
+    int load(int which, const ppg_sdtree &in, uint32_t nodeCap = 0) {
+        const size_t n = in.n_nodes;
+        if (n >= 0xFFFFFFFFull) return fail(PPG_ERR_INVALID_ARGUMENT, "more S-tree nodes than 32-bit node numbers hold");
+        std::vector<uint32_t> first(n, 0u); std::vector<float4> la(n);
+        for (size_t i = 0; i < n; ++i) {
+            if (in.tree_first && in.tree_first[i] > 0xFFFFFFFFull) return fail(PPG_ERR_INVALID_ARGUMENT, "tree_first past the 32 bits of the leaf record");
+            if (in.tree_first) first[i] = (uint32_t) in.tree_first[i];
+            const bool valid = !which && dtree_mean(in.tree_sum ? in.tree_sum[i] : 0.f, in.tree_weight ? in.tree_weight[i] : 0.f) > 0.f;
+            la[i] = make_float4(bits_f(first[i]), which ? bits_f(first[i]) : 0.f, in.adam ? in.adam[6 * i + 3] : 0.f, bits_f(valid ? 1u : 0u));
+        }
         int dev = 0;
         CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev)); CK(dStable.alloc(kTableEntries));
-        int rc = reserve(std::max<uint32_t>(nodeCap, 1), std::max<size_t>(nPool, 1), true); if (rc) return rc;
-        std::vector<float4> la(n);
-        for (size_t i = 0; i < n; ++i) {
-            const float f = bits_f(first ? first[i] : 0u);
-            la[i] = make_float4(f, which ? f : 0.f, adam ? adam[6 * i + 3] : 0.f, 0.f);
-        }
-        CK(put(dSnodes, nodeChildren, n)); CK(put(dLeafA, la.data(), n)); CK(put(dAdam, adam, 6 * n)); CK(put(dSampSum, sum, n));
-        CK(put(dSampWeight, which ? nullptr : weight, n)); CK(put(dSampCount, which ? nullptr : count, n)); CK(put(dSampDepth, which ? nullptr : depth, n));
-        CK(put(dBweight, which ? weight : nullptr, n)); CK(put(dBuildCount, which ? count : nullptr, n)); CK(put(dBuildDepth, which ? depth : nullptr, n));
-        CK(put(dBuildBase, which ? first : nullptr, n));
-        const std::vector<SampNode> pool = which ? std::vector<SampNode>() : to_pool(sums, children, nPool);
-        // the building pool's children keep the ABI's bytes: uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
-        CK(put(dSamp, pool.data(), pool.size())); CK(put(dBchildren, which ? children : nullptr, nPool)); CK(put(dTrain, which ? sums : nullptr, 4 * nPool));
+        int rc = reserve(std::max<uint32_t>(std::max<uint32_t>((uint32_t) n, nodeCap), 1), std::max<size_t>(in.n_pool, 1), true); if (rc) return rc;
+        CK(put(dSnodes, in.node_children, n)); CK(put(dLeafA, la.data(), n)); CK(put(dAdam, in.adam, 6 * n)); CK(put(dSampSum, which ? nullptr : in.tree_sum, n));
+        CK(put(dSampWeight, which ? nullptr : in.tree_weight, n)); CK(put(dSampCount, which ? nullptr : in.tree_count, n)); CK(put(dSampDepth, which ? nullptr : in.tree_depth, n));
+        CK(put(dBweight, which ? in.tree_weight : nullptr, n)); CK(put(dBuildCount, which ? in.tree_count : nullptr, n)); CK(put(dBuildDepth, which ? in.tree_depth : nullptr, n));
+        CK(put(dBuildBase, which ? first.data() : nullptr, n));
+        const std::vector<SampNode> pool = which ? std::vector<SampNode>() : to_pool(in.sums, in.children, in.n_pool);
+        CK(put(dSamp, pool.data(), pool.size())); CK(put(dBchildren, which ? in.children : nullptr, in.n_pool)); CK(put(dTrain, which ? in.sums : nullptr, 4 * in.n_pool));
         const uint32_t sc[8] = {(uint32_t) n, 0, 0, 0, 0, 0, 0, 0};
         CK(put(dScalars, sc, 8));
         hNodes = (uint32_t) n; hTotalBuild = 0;
@@ -390,29 +393,61 @@ struct TreeStore {
         return 1;
     }
 
-    int gather(int which, TreeGather &g, size_t minPool = 1) const {
+    // The sampling (which == 0) or building trees into a caller's ppg_sdtree.  compact: the leaves' quadtrees concatenated in node order and
+    // tree_first counted along them (ppg_export_sdtree: between the reset and the build of an iteration the sampling trees still sit where the
+    // previous build put them, and a leaf the refine made shares its parent's).  Otherwise tree_first is the offset in the device pool, which
+    // is copied from 0 to the end of the last leaf's quadtree: the ops' results keep the offsets the caller loaded.
+    int store(int which, ppg_sdtree &out, bool compact = true) const {
         if (capNodes == 0) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
-        const uint32_t n = g.n = hNodes;
-        g.sn.resize(n); g.la.resize(n); g.sum.assign(n, 0.f); g.weight.resize(n); g.adam.resize(6 * (size_t) n); g.depth.resize(n); g.count.resize(n);
-        CK(cudaMemcpy(g.sn.data(), dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.la.data(), dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.adam.data(), dAdam.p, 24 * (size_t) n, cudaMemcpyDeviceToHost));
-        if (which == 0) CK(cudaMemcpy(g.sum.data(), dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.weight.data(), which ? dBweight.p : dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.depth.data(), which ? dBuildDepth.p : dSampDepth.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(g.count.data(), which ? dBuildCount.p : dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
-        size_t end = minPool;
-        for (uint32_t i = 0; i < n; ++i) if (g.sn[i].x == 0u) end = std::max<size_t>(end, (size_t) g.first(i, which) + g.count[i]);
+        const uint32_t n = hNodes;
+        std::vector<uint2> sn(n); std::vector<float4> la(n); std::vector<float> sum(n, 0.f), weight(n), adam(6 * (size_t) n); std::vector<int> depth(n); std::vector<uint32_t> count(n);
+        CK(cudaMemcpy(sn.data(), dSnodes.p, sizeof(uint2) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(la.data(), dLeafA.p, sizeof(float4) * n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(adam.data(), dAdam.p, 24 * (size_t) n, cudaMemcpyDeviceToHost));
+        if (which == 0) CK(cudaMemcpy(sum.data(), dSampSum.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(weight.data(), which ? dBweight.p : dSampWeight.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(depth.data(), which ? dBuildDepth.p : dSampDepth.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(count.data(), which ? dBuildCount.p : dSampCount.p, 4 * (size_t) n, cudaMemcpyDeviceToHost));
+        const auto first = [&](uint32_t i) { return f_bits(which ? la[i].y : la[i].x); };
+        size_t total = 0, end = 0;
+        for (uint32_t i = 0; i < n; ++i) if (sn[i].x == 0u) { total += count[i]; end = std::max<size_t>(end, (size_t) first(i) + count[i]); }
         if (end > capPool) return fail(PPG_ERR_CUDA, "SD-tree leaf points past the quadtree pool");
-        g.children.resize(end); g.sums.resize(end);
-        if (which) {
-            CK(cudaMemcpy(g.children.data(), dBchildren.p, sizeof(uint2) * end, cudaMemcpyDeviceToHost));
-            CK(cudaMemcpy(g.sums.data(), dTrain.p, sizeof(float4) * end, cudaMemcpyDeviceToHost));
-        } else {
-            std::vector<SampNode> pool(end);
-            CK(cudaMemcpy(pool.data(), dSamp.p, sizeof(SampNode) * end, cudaMemcpyDeviceToHost));
-            for (size_t k = 0; k < end; ++k) { g.children[k] = pool[k].children; g.sums[k] = pool[k].sums; }
+        out.n_nodes = n; out.n_pool = compact ? total : end;
+        if (out.n_nodes > out.node_capacity || out.n_pool > out.pool_capacity)
+            return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_sdtree output arrays too small (n_nodes and n_pool hold the sizes needed)");
+        std::vector<SampNode> pool(end);                // building pool: bsums and bchildren, strided into the sampling pool's layout
+        if (end && (out.sums || out.children)) {
+            if (which) {
+                CK(cudaMemcpy2D(&pool[0].sums, sizeof(SampNode), dTrain.p, sizeof(float4), sizeof(float4), end, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy2D(&pool[0].children, sizeof(SampNode), dBchildren.p, sizeof(uint2), sizeof(uint2), end, cudaMemcpyDeviceToHost));
+            } else CK(cudaMemcpy(pool.data(), dSamp.p, sizeof(SampNode) * end, cudaMemcpyDeviceToHost));
         }
+        const auto row = [&](size_t k, const SampNode &q) {      // children keep their bytes (see to_pool)
+            if (out.sums) memcpy(out.sums + 4 * k, &q.sums, 16);
+            if (out.children) memcpy(out.children + 4 * k, &q.children, 8);
+        };
+        uint64_t off = 0;
+        for (uint32_t i = 0; i < n; ++i) {          // inner nodes carry no tree and no optimiser state (STree::subdivide, GP:876-895)
+            const bool leaf = sn[i].x == 0u;
+            if (out.node_children) memcpy(out.node_children + 2 * (size_t) i, &sn[i], 8);
+            if (out.tree_first) out.tree_first[i] = compact ? off : first(i);
+            if (out.tree_count) out.tree_count[i] = leaf ? count[i] : 0u;
+            if (out.tree_depth) out.tree_depth[i] = leaf ? depth[i] : 0;
+            if (out.tree_sum) out.tree_sum[i] = leaf ? sum[i] : 0.f;
+            if (out.tree_weight) out.tree_weight[i] = leaf ? weight[i] : 0.f;
+            if (out.adam)                           // theta as the bounce kernel reads it
+                for (int j = 0; j < 6; ++j) out.adam[6 * (size_t) i + j] = !leaf ? 0.f : j == 3 ? la[i].z : adam[6 * (size_t) i + j];
+            if (!leaf || !compact) continue;
+            for (uint32_t k = 0; k < count[i]; ++k) row(off + k, pool[first(i) + k]);
+            off += count[i];
+        }
+        if (!compact) for (size_t k = 0; k < end; ++k) row(k, pool[k]);
+        return PPG_OK;
+    }
+    // the building sums and weights a record or commit added to, back into the caller's tree
+    int copy_back(const ppg_sdtree &b) const {
+        if (b.sums) CK(cudaMemcpy(b.sums, dTrain.p, 16 * b.n_pool, cudaMemcpyDeviceToHost));
+        if (b.tree_weight) CK(cudaMemcpy(b.tree_weight, dBweight.p, 4 * b.n_nodes, cudaMemcpyDeviceToHost));
         return PPG_OK;
     }
 };
@@ -1287,45 +1322,16 @@ extern "C" int ppg_get_moment_images(ppg_integrator *h, float *sum_rgbw, float *
     return PPG_OK;
 }
 
-static int gather_tree(ppg_integrator *h, int which, TreeGather &g) {
+static int store_tree(ppg_integrator *h, int which, ppg_sdtree &out) {
     if (!h->haveScene) return fail(PPG_ERR_NO_SCENE, "no SD-tree yet");
     CK(cudaSetDevice(h->device));
-    return h->tree.gather(which, g);
+    return h->tree.store(which, out);
 }
 
-extern "C" int ppg_export_sdtree(ppg_integrator *h, int which, size_t node_capacity, size_t *n_nodes_out, uint32_t *node_children, uint64_t *tree_first,
-                                 uint32_t *tree_count, int32_t *tree_depth, float *tree_sum, float *tree_weight, float *adam,
-                                 size_t pool_capacity, size_t *n_pool_out, float *sums, uint16_t *children, float *aabb_min_max) {
+extern "C" int ppg_export_sdtree(ppg_integrator *h, int which, ppg_sdtree *out, float *aabb_min_max) {
   return guarded("ppg_export_sdtree", [&]() -> int {
-    if (!h || !n_nodes_out || !n_pool_out || (which != 0 && which != 1)) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_export_sdtree: null argument or `which` not 0 / 1");
-    TreeGather g; int rc = gather_tree(h, which, g); if (rc) return rc;
-    size_t total = 0;
-    for (uint32_t i = 0; i < g.n; ++i) if (g.sn[i].x == 0u) total += g.count[i];
-    *n_nodes_out = g.n; *n_pool_out = total;
-    if (g.n > node_capacity || total > pool_capacity)
-        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_export_sdtree: output arrays too small (*n_nodes_out and *n_pool_out hold the sizes needed)");
-    uint64_t off = 0;
-    for (uint32_t i = 0; i < g.n; ++i) {          // inner nodes carry no tree and no optimiser state (STree::subdivide, GP:876-895)
-        const bool leaf = g.sn[i].x == 0u;
-        if (node_children) { node_children[2 * i] = g.sn[i].x; node_children[2 * i + 1] = g.sn[i].y; }
-        if (tree_first) tree_first[i] = off;
-        if (tree_count) tree_count[i] = leaf ? g.count[i] : 0u;
-        if (tree_depth) tree_depth[i] = leaf ? g.depth[i] : 0;
-        if (tree_sum) tree_sum[i] = leaf ? g.sum[i] : 0.f;
-        if (tree_weight) tree_weight[i] = leaf ? g.weight[i] : 0.f;
-        if (adam) {
-            for (int j = 0; j < 6; ++j) adam[6 * (size_t) i + j] = leaf ? g.adam[6 * (size_t) i + j] : 0.f;
-            if (leaf) adam[6 * (size_t) i + 3] = g.la[i].z;           // theta as the bounce kernel reads it
-        }
-        if (!leaf) continue;
-        const uint32_t base = g.first(i, which);
-        for (uint32_t k = 0; k < g.count[i]; ++k) {
-            const float4 s = g.sums[base + k]; const uint2 c = g.children[base + k];
-            if (sums) { float *o = sums + 4 * (off + k); o[0] = s.x; o[1] = s.y; o[2] = s.z; o[3] = s.w; }
-            if (children) { uint16_t *o = children + 4 * (off + k); o[0] = (uint16_t) (c.x & 0xffff); o[1] = (uint16_t) (c.x >> 16); o[2] = (uint16_t) (c.y & 0xffff); o[3] = (uint16_t) (c.y >> 16); }
-        }
-        off += g.count[i];
-    }
+    if (!h || !out || (which != 0 && which != 1)) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_export_sdtree: null argument or `which` not 0 / 1");
+    int rc = store_tree(h, which, *out); if (rc) return rc;
     if (aabb_min_max) {                           // the cubified box of the S-tree (STree::STree, GP:850-860; pack_scene)
         const float m = std::max(std::max(h->aabbMax[0] - h->aabbMin[0], h->aabbMax[1] - h->aabbMin[1]), h->aabbMax[2] - h->aabbMin[2]);
         for (int a = 0; a < 3; ++a) { aabb_min_max[a] = h->aabbMin[a]; aabb_min_max[3 + a] = h->aabbMin[a] + m; }
@@ -1341,8 +1347,15 @@ static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path);
 extern "C" int ppg_dump_sdtree(ppg_integrator *h, const char *path) { return guarded("ppg_dump_sdtree", [&] { return ppg_dump_sdtree_impl(h, path); }); }
 static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path) {
     if (!h || !path) return fail(PPG_ERR_INVALID_ARGUMENT, "null argument");
-    TreeGather g; int rc = gather_tree(h, 0, g); if (rc) return rc;
-    const std::vector<uint2> &sn = g.sn; const std::vector<float> &ssum = g.sum, &sw = g.weight; const std::vector<uint32_t> &scnt = g.count;
+    ppg_sdtree t = {};
+    int rc = store_tree(h, 0, t);                 // no room (an S-tree has a node): only the sizes
+    if (rc != PPG_ERR_INVALID_ARGUMENT) return rc;
+    std::vector<uint32_t> sn(2 * t.n_nodes), count(t.n_nodes); std::vector<uint64_t> first(t.n_nodes); std::vector<float> sum(t.n_nodes), weight(t.n_nodes);
+    std::vector<float> sums(4 * t.n_pool); std::vector<uint16_t> children(4 * t.n_pool);
+    t.node_capacity = t.n_nodes; t.pool_capacity = t.n_pool;
+    t.node_children = sn.data(); t.tree_first = first.data(); t.tree_count = count.data(); t.tree_sum = sum.data(); t.tree_weight = weight.data();
+    t.sums = sums.data(); t.children = children.data();
+    rc = store_tree(h, 0, t); if (rc) return rc;
     FILE *f = fopen(path, "wb");
     if (!f) return fail(PPG_ERR_IO, std::string("cannot open ") + path);
     float cm[16];
@@ -1356,23 +1369,17 @@ static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path) {
     st.push_back(root);
     while (!st.empty()) {
         E e = st.back(); st.pop_back();
-        if (sn[e.n].x == 0u) {
-            if (!(sw[e.n] > 0)) continue;
-            const float mean = (1 / (3.14159265358979323846f * 4 * sw[e.n])) * ssum[e.n];
+        if (sn[2 * e.n] == 0u) {
+            if (!(weight[e.n] > 0)) continue;
+            const float mean = (1 / (3.14159265358979323846f * 4 * weight[e.n])) * sum[e.n];
             fwrite(e.p, 4, 3, f); fwrite(e.s, 4, 3, f); fwrite(&mean, 4, 1, f);
-            const uint64_t w64 = (uint64_t) sw[e.n], nn = scnt[e.n];
+            const uint64_t w64 = (uint64_t) weight[e.n], nn = count[e.n];
             fwrite(&w64, 8, 1, f); fwrite(&nn, 8, 1, f);
-            const uint32_t base = g.first(e.n, 0);
-            for (uint32_t k = 0; k < scnt[e.n]; ++k) {
-                const float4 &s = g.sums[base + k]; const uint2 &c = g.children[base + k];
-                const float s4[4] = {s.x, s.y, s.z, s.w};
-                const uint16_t c4[4] = {(uint16_t) (c.x & 0xffff), (uint16_t) (c.x >> 16), (uint16_t) (c.y & 0xffff), (uint16_t) (c.y >> 16)};
-                for (int j = 0; j < 4; ++j) { fwrite(&s4[j], 4, 1, f); fwrite(&c4[j], 2, 1, f); }
-            }
+            for (uint64_t k = 4 * first[e.n]; k < 4 * (first[e.n] + nn); ++k) { fwrite(&sums[k], 4, 1, f); fwrite(&children[k], 2, 1, f); }
         } else {
             E a = e, b = e;
             a.s[e.axis] = b.s[e.axis] = e.s[e.axis] / 2; b.p[e.axis] += b.s[e.axis];
-            a.axis = b.axis = (e.axis + 1) % 3; a.n = sn[e.n].x; b.n = sn[e.n].y;
+            a.axis = b.axis = (e.axis + 1) % 3; a.n = sn[2 * e.n]; b.n = sn[2 * e.n + 1];
             st.push_back(b); st.push_back(a);
         }
     }
@@ -1384,20 +1391,23 @@ static int ppg_dump_sdtree_impl(ppg_integrator *h, const char *path) {
 namespace {
 struct ReplayRng { const float *v; uint32_t n, i; __device__ float next1D() { return i < n ? v[i++] : 0.5f; } };
 
-__global__ void op_pdf_kernel(const SampNode *pool, const uint32_t *first, const float *tsum, const float *tweight, const uint32_t *qt, const float *qd, size_t n, float *out) {
+// the sampling tree of node t as the bounce kernel reads it
+__device__ __forceinline__ const SampNode *op_tree(const TreeView &T, uint32_t t, bool &valid) {
+    const float4 la = T.leafA[t];
+    valid = __float_as_uint(la.w) & 1u;
+    return T.samp + __float_as_uint(la.x);
+}
+__global__ void op_pdf_kernel(const __grid_constant__ TreeView T, const uint32_t *qt, const float *qd, size_t n, float *out) {
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
-        const uint32_t t = qt[i];
-        float mean = 0.f; if (tweight[t] != 0.f) mean = (1.f / (PPG_PI * 4.f * tweight[t])) * tsum[t];
-        out[i] = dtree_pdf(pool + first[t], mean > 0.f, dir_to_canonical(f3(qd[3 * i], qd[3 * i + 1], qd[3 * i + 2])));
+        bool valid; const SampNode *tree = op_tree(T, qt[i], valid);
+        out[i] = dtree_pdf(tree, valid, dir_to_canonical(f3(qd[3 * i], qd[3 * i + 1], qd[3 * i + 2])));
     }
 }
-__global__ void op_sample_kernel(const SampNode *pool, const uint32_t *first, const float *tsum, const float *tweight, const uint32_t *qt, const float *rnd, size_t stride, size_t n, float *out,
-                                 float *canon) {
+__global__ void op_sample_kernel(const __grid_constant__ TreeView T, const uint32_t *qt, const float *rnd, size_t stride, size_t n, float *out, float *canon) {
     for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
-        const uint32_t t = qt[i];
-        float mean = 0.f; if (tweight[t] != 0.f) mean = (1.f / (PPG_PI * 4.f * tweight[t])) * tsum[t];
+        bool valid; const SampNode *tree = op_tree(T, qt[i], valid);
         ReplayRng r{rnd + stride * i, (uint32_t) stride, 0u};
-        const float2 c = dtree_sample(pool + first[t], mean > 0.f, r);
+        const float2 c = dtree_sample(tree, valid, r);
         const float3 d = canonical_to_dir(c);
         out[3 * i] = d.x; out[3 * i + 1] = d.y; out[3 * i + 2] = d.z;
         if (canon) { canon[2 * i] = c.x; canon[2 * i + 1] = c.y; }
@@ -1460,56 +1470,52 @@ static int op_device(int device) {
 }
 }  // namespace
 
-extern "C" int ppg_op_dtree_pdf(int device, const float *sums, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
-                                const float *tree_sum, const float *tree_weight, size_t n_trees, const uint32_t *query_tree, const float *query_dir,
-                                size_t n, float *pdf_out) {
+static const float kNoBox[3] = {0.f, 0.f, 0.f};     // the D-tree ops look up no point
+
+extern "C" int ppg_op_dtree_pdf(int device, const ppg_sdtree *tree, const uint32_t *query_tree, const float *query_dir, size_t n, float *pdf_out) {
+  return guarded("ppg_op_dtree_pdf", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    std::vector<SampNode> pool = to_pool(sums, children, n_nodes);
-    Up<SampNode> dp; Up<uint32_t> df, dq; Up<float> ds, dw, dd; DevBuf<float> out;
-    if (dp.up(pool.data(), n_nodes) || df.up(tree_first_node, n_trees) || ds.up(tree_sum, n_trees) || dw.up(tree_weight, n_trees) || dq.up(query_tree, n) || dd.up(query_dir, 3 * n))
-        return fail(PPG_ERR_CUDA, "upload failed");
+    if (!tree) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_dtree_pdf: null tree");
+    TreeStore t; rc = t.load(0, *tree); if (rc) return rc;
+    Up<uint32_t> dq; Up<float> dd; DevBuf<float> out;
+    if (dq.up(query_tree, n) || dd.up(query_dir, 3 * n)) return fail(PPG_ERR_CUDA, "upload failed");
     CK(out.alloc(std::max<size_t>(n, 1)));
-    if (n) op_pdf_kernel<<<296, 256>>>(dp.b.p, df.b.p, ds.b.p, dw.b.p, dq.b.p, dd.b.p, n, out.p);
+    if (n) op_pdf_kernel<<<296, 256>>>(t.view(kNoBox, kNoBox), dq.b.p, dd.b.p, n, out.p);
     CK(cudaGetLastError());
     CK(cudaMemcpy(pdf_out, out.p, 4 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
+  });
 }
-extern "C" int ppg_op_dtree_sample(int device, const float *sums, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
-                                   const float *tree_sum, const float *tree_weight, size_t n_trees, const uint32_t *query_tree, const float *rnd,
-                                   size_t rnd_stride, size_t n, float *dir_out, float *canonical_out) {
+extern "C" int ppg_op_dtree_sample(int device, const ppg_sdtree *tree, const uint32_t *query_tree, const float *rnd, size_t rnd_stride, size_t n,
+                                   float *dir_out, float *canonical_out) {
+  return guarded("ppg_op_dtree_sample", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    std::vector<SampNode> pool = to_pool(sums, children, n_nodes);
-    Up<SampNode> dp; Up<uint32_t> df, dq; Up<float> ds, dw, dr; DevBuf<float> out, canon;
-    if (dp.up(pool.data(), n_nodes) || df.up(tree_first_node, n_trees) || ds.up(tree_sum, n_trees) || dw.up(tree_weight, n_trees) || dq.up(query_tree, n) || dr.up(rnd, rnd_stride * n))
-        return fail(PPG_ERR_CUDA, "upload failed");
+    if (!tree) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_dtree_sample: null tree");
+    TreeStore t; rc = t.load(0, *tree); if (rc) return rc;
+    Up<uint32_t> dq; Up<float> dr; DevBuf<float> out, canon;
+    if (dq.up(query_tree, n) || dr.up(rnd, rnd_stride * n)) return fail(PPG_ERR_CUDA, "upload failed");
     CK(out.alloc(std::max<size_t>(3 * n, 1)));
     if (canonical_out) CK(canon.alloc(std::max<size_t>(2 * n, 1)));
-    if (n) op_sample_kernel<<<296, 256>>>(dp.b.p, df.b.p, ds.b.p, dw.b.p, dq.b.p, dr.b.p, rnd_stride, n, out.p, canon.p);
+    if (n) op_sample_kernel<<<296, 256>>>(t.view(kNoBox, kNoBox), dq.b.p, dr.b.p, rnd_stride, n, out.p, canon.p);
     CK(cudaGetLastError());
     CK(cudaMemcpy(dir_out, out.p, 12 * n, cudaMemcpyDeviceToHost));
     if (canonical_out) CK(cudaMemcpy(canonical_out, canon.p, 8 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
+  });
 }
-extern "C" int ppg_op_dtree_record(int device, float *sums_inout, const uint16_t *children, size_t n_nodes, const uint32_t *tree_first_node,
-                                   float *tree_weight_inout, size_t n_trees, const uint32_t *rec_tree, const float *rec_dir, const float *rec_radiance,
+extern "C" int ppg_op_dtree_record(int device, const ppg_sdtree *tree, const uint32_t *rec_tree, const float *rec_dir, const float *rec_radiance,
                                    const float *rec_wo_pdf, const float *rec_weight, size_t n, int filter) {
+  return guarded("ppg_op_dtree_record", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    std::vector<uint2> bch(n_nodes);
-    for (size_t i = 0; i < n_nodes; ++i)
-        bch[i] = make_uint2((uint32_t) children[4 * i] | ((uint32_t) children[4 * i + 1] << 16), (uint32_t) children[4 * i + 2] | ((uint32_t) children[4 * i + 3] << 16));
-    std::vector<float4> la(n_trees);
-    for (size_t t = 0; t < n_trees; ++t) { uint32_t b = tree_first_node[t]; float fb; memcpy(&fb, &b, 4); la[t] = make_float4(fb, fb, 0.f, 0.f); }
-    Up<uint2> dch; Up<float4> dla; Up<float> dsums, dwt, dd, drad, dpdf, dw; Up<uint32_t> drt;
-    if (dch.up(bch.data(), n_nodes) || dla.up(la.data(), n_trees) || dsums.up(sums_inout, 4 * n_nodes) || dwt.up(tree_weight_inout, n_trees) || drt.up(rec_tree, n) ||
-        dd.up(rec_dir, 3 * n) || drad.up(rec_radiance, n) || dpdf.up(rec_wo_pdf, n) || dw.up(rec_weight, n))
+    if (!tree) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_dtree_record: null tree");
+    TreeStore t; rc = t.load(1, *tree); if (rc) return rc;
+    Up<float> dd, drad, dpdf, dw; Up<uint32_t> drt;
+    if (drt.up(rec_tree, n) || dd.up(rec_dir, 3 * n) || drad.up(rec_radiance, n) || dpdf.up(rec_wo_pdf, n) || dw.up(rec_weight, n))
         return fail(PPG_ERR_CUDA, "upload failed");
-    TreeView T; memset(&T, 0, sizeof(T));
-    T.leafA = dla.b.p; T.bchildren = dch.b.p; T.bsums = reinterpret_cast<float4 *>(dsums.b.p); T.bweight = dwt.b.p;
-    if (n) op_record_kernel<<<296, 256>>>(T, drt.b.p, dd.b.p, drad.b.p, dpdf.b.p, dw.b.p, n, filter);
+    if (n) op_record_kernel<<<296, 256>>>(t.view(kNoBox, kNoBox), drt.b.p, dd.b.p, drad.b.p, dpdf.b.p, dw.b.p, n, filter);
     CK(cudaGetLastError());
-    CK(cudaMemcpy(sums_inout, dsums.b.p, 16 * n_nodes, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(tree_weight_inout, dwt.b.p, 4 * n_trees, cudaMemcpyDeviceToHost));
-    return PPG_OK;
+    return t.copy_back(*tree);
+  });
 }
 // The acceleration structure ppg_set_scene builds, on the host alone (no CUDA device needed): for tests of the builder and for timing it.
 extern "C" int ppg_op_bvh_build(const float *positions, const uint32_t *indices, size_t n_triangles, int threads, float *nodes_out, size_t nodes_capacity,
@@ -1557,13 +1563,12 @@ extern "C" int ppg_op_env_pdf(ppg_integrator *h, size_t n, const float *d, float
     if (value_out) CK(cudaMemcpy(value_out, ov.p, 12 * n, cudaMemcpyDeviceToHost));
     return PPG_OK;
 }
-extern "C" int ppg_op_stree_lookup(int device, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
+extern "C" int ppg_op_stree_lookup(int device, const ppg_sdtree *tree, const float aabb_min[3], const float aabb_extent[3],
                                    const float *points, size_t n, uint32_t *leaf_out, float *size_out) {
   return guarded("ppg_op_stree_lookup", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    if (n_nodes >= 0xFFFFFFFFull) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_stree_lookup: more S-tree nodes than 32-bit node numbers hold");
-    TreeStore t;
-    rc = t.load(0, n_nodes, (uint32_t) n_nodes, node_children, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr); if (rc) return rc;
+    if (!tree) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_stree_lookup: null tree");
+    TreeStore t; rc = t.load(0, *tree); if (rc) return rc;
     Up<float> dp; DevBuf<uint32_t> dl; DevBuf<float> dsz;
     if (dp.up(points, 3 * n)) return fail(PPG_ERR_CUDA, "upload failed");
     CK(dl.alloc(std::max<size_t>(n, 1))); CK(dsz.alloc(std::max<size_t>(3 * n, 1)));
@@ -1580,73 +1585,45 @@ extern "C" int ppg_op_stree_lookup(int device, const uint32_t *node_children, si
 // ------------------------------------------------------------------ the learning half: the render's own maintenance, commit and Adam launches (TreeStore)
 
 extern "C" int ppg_op_sdtree_refine_reset(int device, int stages, float threshold, int new_max_depth, float dtree_threshold, size_t node_capacity,
-                                          const uint32_t *node_children, size_t n_nodes, const uint32_t *tree_first, const uint32_t *tree_count, const int32_t *tree_depth,
-                                          const float *tree_sum, const float *tree_weight, const float *adam, const float *building_weight,
-                                          const float *sums, const uint16_t *children, size_t n_pool,
-                                          size_t out_capacity, size_t *n_nodes_out, uint32_t *node_children_out, uint32_t *tree_first_out, uint32_t *tree_count_out,
-                                          int32_t *tree_depth_out, float *tree_sum_out, float *tree_weight_out, float *adam_out, float *building_weight_out,
-                                          uint32_t *build_first_out, uint32_t *build_count_out, int32_t *build_depth_out,
-                                          size_t build_capacity, size_t *n_build_out, uint16_t *build_children_out, float *build_sums_out) {
+                                          const ppg_sdtree *in, const float *building_weight, ppg_sdtree *sampling_out, ppg_sdtree *building_out) {
   return guarded("ppg_op_sdtree_refine_reset", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    if (!n_nodes || n_nodes >= 0xFFFFFFFFull || !node_children || !tree_first || !tree_count || !tree_depth || !tree_sum || !tree_weight || !adam || !building_weight ||
-        !sums || !children || !n_pool || !n_nodes_out || !n_build_out)
-        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: empty or null input");
+    if (!in || !in->n_nodes || !building_weight || !sampling_out || !building_out) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: empty or null input");
+    const size_t n_nodes = in->n_nodes;
     double totalW = 0; for (size_t i = 0; i < n_nodes; ++i) totalW += building_weight[i];
     const uint32_t cap = node_capacity ? (uint32_t) std::min<size_t>(node_capacity, 0xFFFFFFFFull)
                                        : std::max<uint32_t>((uint32_t) std::min<double>(refine_capacity(n_nodes, 1.25 * totalW + 4096, threshold), 4.0e9), 1u << 16);
     if (cap < n_nodes) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: node_capacity below n_nodes");
-    TreeStore t;
-    rc = t.load(0, n_nodes, cap, node_children, tree_first, tree_count, tree_depth, tree_sum, tree_weight, adam, n_pool, sums, children); if (rc) return rc;
+    TreeStore t; rc = t.load(0, *in, cap); if (rc) return rc;
     CK(t.put(t.dBweight, building_weight, n_nodes));
     if (stages & 1) t.refine(threshold);
     if (stages & 2) t.reset_count(new_max_depth, dtree_threshold);
     CK(cudaGetLastError());
     rc = t.sync_counts(true); if (rc) return rc;
-    const size_t N = t.hNodes, total = t.hTotalBuild;
-    *n_nodes_out = N; *n_build_out = total;
-    if (N > out_capacity || total > build_capacity)
-        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: output arrays too small (*n_nodes_out and *n_build_out hold the sizes needed)");
-    if (building_weight_out) CK(cudaMemcpy(building_weight_out, t.dBweight.p, 4 * N, cudaMemcpyDeviceToHost));      // reset_fill zeroes it
+    building_out->n_nodes = t.hNodes; building_out->n_pool = t.hTotalBuild;
+    rc = t.store(0, *sampling_out, false);        // the refine's result: the reset changes no sampling tree
+    if (rc || t.hNodes > building_out->node_capacity || t.hTotalBuild > building_out->pool_capacity)
+        return rc ? rc : fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_refine_reset: building_out too small (its n_nodes and n_pool hold the sizes needed)");
+    if (building_out->tree_weight) CK(cudaMemcpy(building_out->tree_weight, t.dBweight.p, 4 * (size_t) t.hNodes, cudaMemcpyDeviceToHost));     // reset_fill clears it
     if (stages & 2) t.reset_fill(new_max_depth, dtree_threshold);
     CK(cudaGetLastError());
-    std::vector<float4> laOut(N); CK(cudaMemcpy(laOut.data(), t.dLeafA.p, 16 * N, cudaMemcpyDeviceToHost));
-    if (tree_first_out) for (size_t i = 0; i < N; ++i) tree_first_out[i] = f_bits(laOut[i].x);
-    if (node_children_out) CK(cudaMemcpy(node_children_out, t.dSnodes.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (tree_count_out) CK(cudaMemcpy(tree_count_out, t.dSampCount.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_depth_out) CK(cudaMemcpy(tree_depth_out, t.dSampDepth.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_sum_out) CK(cudaMemcpy(tree_sum_out, t.dSampSum.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (tree_weight_out) CK(cudaMemcpy(tree_weight_out, t.dSampWeight.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (adam_out) CK(cudaMemcpy(adam_out, t.dAdam.p, 24 * N, cudaMemcpyDeviceToHost));
-    if (build_first_out) CK(cudaMemcpy(build_first_out, t.dBuildBase.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_count_out) CK(cudaMemcpy(build_count_out, t.dBuildCount.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_depth_out) CK(cudaMemcpy(build_depth_out, t.dBuildDepth.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (build_children_out && total) CK(cudaMemcpy(build_children_out, t.dBchildren.p, 8 * total, cudaMemcpyDeviceToHost));     // uint2 {c0 | c1 << 16, c2 | c3 << 16} == 4 x uint16
-    if (build_sums_out && total) CK(cudaMemcpy(build_sums_out, t.dTrain.p, 16 * total, cudaMemcpyDeviceToHost));
-    return PPG_OK;
+    ppg_sdtree b = *building_out; b.tree_weight = nullptr;
+    return t.store(1, b, false);
   });
 }
 
-extern "C" int ppg_op_sdtree_build(int device, const uint32_t *node_children, size_t n_nodes, const uint32_t *build_first, const uint32_t *build_count,
-                                   const int32_t *build_depth, const float *building_weight, const float *sums, const uint16_t *children, size_t n_pool,
-                                   float *sampling_sums_out, uint16_t *sampling_children_out, float *tree_sum_out, float *tree_weight_out,
-                                   int32_t *tree_depth_out, uint32_t *tree_count_out, uint8_t *mean_positive_out, double *stats_out) {
+extern "C" int ppg_op_sdtree_build(int device, const ppg_sdtree *building, ppg_sdtree *sampling_out, uint8_t *mean_positive_out, double *stats_out) {
   return guarded("ppg_op_sdtree_build", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
-    if (!n_nodes || n_nodes >= 0xFFFFFFFFull || !node_children || !build_first || !build_count || !build_depth || !building_weight || !sums || !children || !n_pool)
-        return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_build: empty or null input");
-    TreeStore t; rc = t.load(1, n_nodes, (uint32_t) n_nodes, node_children, build_first, build_count, build_depth, nullptr, building_weight, nullptr, n_pool, sums, children);
-    if (rc) return rc;
+    if (!building || !building->n_nodes || !sampling_out) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_sdtree_build: empty or null input");
+    TreeStore t; rc = t.load(1, *building); if (rc) return rc;
     t.build(); t.tree_stats();
     CK(cudaGetLastError());
-    TreeGather g; rc = t.gather(0, g, n_pool); if (rc) return rc;
-    if (sampling_sums_out) memcpy(sampling_sums_out, g.sums.data(), 16 * n_pool);
-    if (sampling_children_out) memcpy(sampling_children_out, g.children.data(), 8 * n_pool);
-    if (tree_sum_out) memcpy(tree_sum_out, g.sum.data(), 4 * n_nodes);
-    if (tree_weight_out) memcpy(tree_weight_out, g.weight.data(), 4 * n_nodes);
-    if (tree_depth_out) memcpy(tree_depth_out, g.depth.data(), 4 * n_nodes);
-    if (tree_count_out) memcpy(tree_count_out, g.count.data(), 4 * n_nodes);
-    if (mean_positive_out) for (size_t i = 0; i < n_nodes; ++i) mean_positive_out[i] = f_bits(g.la[i].w) != 0u;
+    rc = t.store(0, *sampling_out, false); if (rc) return rc;
+    if (mean_positive_out) {
+        std::vector<float4> la(t.hNodes); CK(cudaMemcpy(la.data(), t.dLeafA.p, sizeof(float4) * la.size(), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < la.size(); ++i) mean_positive_out[i] = f_bits(la[i].w) != 0u;
+    }
     if (stats_out) {
         TreeStats s; CK(cudaMemcpy(&s, t.dTreeStats.p, sizeof(s), cudaMemcpyDeviceToHost));
         const double v[14] = {(double) s.leaves, (double) s.leavesWithNodes, (double) s.depthMin, (double) s.depthMax, s.meanMin, s.meanMax, s.weightMin, s.weightMax,
@@ -1657,18 +1634,15 @@ extern "C" int ppg_op_sdtree_build(int device, const uint32_t *node_children, si
   });
 }
 
-extern "C" int ppg_op_commit(int device, int record_mode, const uint32_t *node_children, size_t n_nodes, const float aabb_min[3], const float aabb_extent[3],
-                             const uint32_t *build_first, float *building_weight_inout, float *sums_inout, const uint16_t *children, size_t n_pool,
+extern "C" int ppg_op_commit(int device, int record_mode, const ppg_sdtree *building, const float aabb_min[3], const float aabb_extent[3],
                              const float *vertices, size_t n, const float *li_final, size_t n_li, int spatial_filter, int directional_filter, int loss,
                              uint64_t seed, float statistical_weight, float *adam_records_out, size_t adam_capacity, size_t *n_adam_out) {
   return guarded("ppg_op_commit", [&]() -> int {
     int rc = op_device(device); if (rc) return rc;
     if (record_mode != 1 && record_mode != 2) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_commit: record_mode is 1 (nearest, 3 vertex fields) or 2 (6 fields)");
-    if (!n_nodes || !node_children || !aabb_min || !aabb_extent || !build_first || !building_weight_inout || !sums_inout || !children || !n_pool ||
-        (n && (!vertices || !li_final)) || n >= 0x40000000ull || !n_adam_out)
+    if (!building || !building->n_nodes || !building->n_pool || !aabb_min || !aabb_extent || (n && (!vertices || !li_final)) || n >= 0x40000000ull || !n_adam_out)
         return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_commit: empty or null input");
-    TreeStore t; rc = t.load(1, n_nodes, (uint32_t) n_nodes, node_children, build_first, nullptr, nullptr, nullptr, building_weight_inout, nullptr, n_pool, sums_inout, children);
-    if (rc) return rc;
+    TreeStore t; rc = t.load(1, *building); if (rc) return rc;
     t.adamCap = std::min<size_t>(adam_capacity, 0xFFFFFFFFull); CK(t.dAdamRecA.alloc(t.adamCap)); CK(t.dAdamRecB.alloc(t.adamCap));
     // the bounce kernel's slab layout: field f of vertex i at f * n + i
     std::vector<float4> slab(6 * std::max<size_t>(n, 1));
@@ -1688,17 +1662,11 @@ extern "C" int ppg_op_commit(int device, int record_mode, const uint32_t *node_c
     C.nee0 = S; C.nSlabs = 1; C.seed = seed; C.dropped = dDrop.b.p;
     if (n) t.commit(C, record_mode, live, 1);
     CK(cudaGetLastError());
-    CK(cudaMemcpy(sums_inout, t.dTrain.p, 16 * n_pool, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(building_weight_inout, t.dBweight.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
+    rc = t.copy_back(*building); if (rc) return rc;
     uint32_t tot = 0; CK(cudaMemcpy(&tot, t.dScalars.p + 3, 4, cudaMemcpyDeviceToHost));
     *n_adam_out = tot;
     const size_t kept = std::min<size_t>(tot, t.adamCap);
-    if (adam_records_out && kept) {
-        std::vector<float4> ra(kept); std::vector<float2> rb(kept);
-        CK(cudaMemcpy(ra.data(), t.dAdamRecA.p, 16 * kept, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), t.dAdamRecB.p, 8 * kept, cudaMemcpyDeviceToHost));
-        for (size_t i = 0; i < kept; ++i) { memcpy(adam_records_out + 6 * i, &ra[i], 16); memcpy(adam_records_out + 6 * i + 4, &rb[i], 8); }
-    }
-    return PPG_OK;
+    return adam_records_out && kept ? records_join(t.dAdamRecA.p, t.dAdamRecB.p, kept, adam_records_out) : PPG_OK;
   });
 }
 
@@ -1713,11 +1681,10 @@ extern "C" int ppg_op_adam_replay(int device, int loss, int bucket, float *state
     if (!bucket)
         for (size_t i = 0; i < n_nodes; ++i)
             if ((size_t) leaf_offset[i] + leaf_count[i] > n_records) return fail(PPG_ERR_INVALID_ARGUMENT, "ppg_op_adam_replay: a leaf's records run past n_records");
-    TreeStore t;
-    rc = t.load(0, n_nodes, (uint32_t) n_nodes, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, state_inout, 0, nullptr, nullptr); if (rc) return rc;
+    ppg_sdtree s = {}; s.n_nodes = s.node_capacity = n_nodes; s.adam = state_inout;
+    TreeStore t; rc = t.load(0, s); if (rc) return rc;
     t.adamCap = n_records; CK(t.dAdamRecA.alloc(n_records)); CK(t.dAdamRecB.alloc(n_records)); CK(t.dAdamSortA.alloc(n_records)); CK(t.dAdamSortB.alloc(n_records));
-    std::vector<float4> ra(n_records); std::vector<float2> rb(n_records);
-    for (size_t i = 0; i < n_records; ++i) { memcpy(&ra[i], records + 6 * i, 16); memcpy(&rb[i], records + 6 * i + 4, 8); }
+    std::vector<float4> ra; std::vector<float2> rb; records_split(records, n_records, ra, rb);
     // records to bucket go where commit appends them; records already grouped go straight into the buckets
     const uint32_t nRec = (uint32_t) n_records;
     CK(cudaMemcpy(t.dScalars.p + 3, &nRec, 4, cudaMemcpyHostToDevice));
@@ -1726,10 +1693,7 @@ extern "C" int ppg_op_adam_replay(int device, int loss, int bucket, float *state
     if (bucket) {
         t.adam_bucket();
         CK(cudaGetLastError());
-        if (bucketed_out && n_records) {
-            CK(cudaMemcpy(ra.data(), t.dAdamSortA.p, 16 * n_records, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(rb.data(), t.dAdamSortB.p, 8 * n_records, cudaMemcpyDeviceToHost));
-            for (size_t i = 0; i < n_records; ++i) { memcpy(bucketed_out + 6 * i, &ra[i], 16); memcpy(bucketed_out + 6 * i + 4, &rb[i], 8); }
-        }
+        if (bucketed_out && n_records) { rc = records_join(t.dAdamSortA.p, t.dAdamSortB.p, n_records, bucketed_out); if (rc) return rc; }
         if (leaf_offset_out) CK(cudaMemcpy(leaf_offset_out, t.dAdamOffset.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
     } else {            // the cursors hold the counts, as after adam_scatter_kernel
         CK(cudaMemcpy(t.dAdamCount.p, leaf_count, 4 * n_nodes, cudaMemcpyHostToDevice)); CK(cudaMemcpy(t.dAdamCursor.p, leaf_count, 4 * n_nodes, cudaMemcpyHostToDevice));
@@ -1738,9 +1702,8 @@ extern "C" int ppg_op_adam_replay(int device, int loss, int bucket, float *state
     }
     t.adam_replay(loss);
     CK(cudaGetLastError());
-    TreeGather g; rc = t.gather(0, g); if (rc) return rc;
-    memcpy(state_inout, g.adam.data(), 24 * n_nodes);
-    if (theta_out) for (size_t i = 0; i < n_nodes; ++i) theta_out[i] = g.la[i].z;
+    rc = t.store(0, s); if (rc) return rc;
+    if (theta_out) for (size_t i = 0; i < n_nodes; ++i) theta_out[i] = state_inout[6 * i + 3];
     if (count_out) CK(cudaMemcpy(count_out, t.dAdamCount.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
     if (cursor_out) CK(cudaMemcpy(cursor_out, t.dAdamCursor.p, 4 * n_nodes, cudaMemcpyDeviceToHost));
     return PPG_OK;

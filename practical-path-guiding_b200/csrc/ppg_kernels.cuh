@@ -388,9 +388,7 @@ __global__ void __launch_bounds__(128) dtree_build_kernel(const __grid_constant_
         float sum = 0.f; sum += r.x; sum += r.y; sum += r.z; sum += r.w;
         const float w = M.bweight[leaf];
         M.sampSum[leaf] = sum; M.sampWeight[leaf] = w; M.sampDepth[leaf] = M.buildDepth[leaf]; M.sampCount[leaf] = count;
-        // DTree::mean() > 0 (GP:387-393)
-        float mean = 0.f;
-        if (w != 0.f) { const float factor = 1.f / (PPG_PI * 4.f * w); mean = factor * sum; }
+        const float mean = dtree_mean(sum, w);
         float4 la = M.leafA[leaf];
         la.x = __uint_as_float(base); la.y = __uint_as_float(base); la.w = __uint_as_float(mean > 0.f ? 1u : 0u);
         M.leafA[leaf] = la;

@@ -107,6 +107,13 @@ class PpgStats(C.Structure):
         return d
 
 
+class PpgSdtree(C.Structure):
+    _fields_ = [("n_nodes", C.c_size_t), ("node_capacity", C.c_size_t), ("node_children", C.POINTER(C.c_uint32)), ("tree_first", C.POINTER(C.c_uint64)),
+                ("tree_count", C.POINTER(C.c_uint32)), ("tree_depth", C.POINTER(C.c_int32)), ("tree_sum", C.POINTER(C.c_float)),
+                ("tree_weight", C.POINTER(C.c_float)), ("adam", C.POINTER(C.c_float)), ("n_pool", C.c_size_t), ("pool_capacity", C.c_size_t),
+                ("sums", C.POINTER(C.c_float)), ("children", C.POINTER(C.c_uint16))]
+
+
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
 CLOCK_FN = C.CFUNCTYPE(C.c_double, C.c_void_p)
 FILM_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int)
@@ -216,22 +223,20 @@ def load_library(path: str | None = None):
     lib.ppg_dump_sdtree.argtypes = [H, C.c_char_p]
     lib.ppg_set_destination.argtypes = [H, C.c_char_p]
     lib.ppg_get_moment_images.argtypes = [H, C.POINTER(C.c_float), C.POINTER(C.c_float)]
-    u16p = C.POINTER(C.c_uint16); u32p = C.POINTER(C.c_uint32); f32p = C.POINTER(C.c_float)
-    lib.ppg_export_sdtree.argtypes = [H, C.c_int, C.c_size_t, C.POINTER(C.c_size_t), u32p, C.POINTER(C.c_uint64), u32p, C.POINTER(C.c_int32), f32p, f32p, f32p,
-                                      C.c_size_t, C.POINTER(C.c_size_t), f32p, u16p, f32p]
-    lib.ppg_op_dtree_pdf.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, f32p, C.c_size_t, u32p, f32p, C.c_size_t, f32p]
-    lib.ppg_op_dtree_sample.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, f32p, C.c_size_t, u32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p]
-    lib.ppg_op_dtree_record.argtypes = [C.c_int, f32p, u16p, C.c_size_t, u32p, f32p, C.c_size_t, u32p, f32p, f32p, f32p, f32p, C.c_size_t, C.c_int]
-    lib.ppg_op_stree_lookup.argtypes = [C.c_int, u32p, C.c_size_t, f32p, f32p, f32p, C.c_size_t, u32p, f32p]
+    u32p = C.POINTER(C.c_uint32); f32p = C.POINTER(C.c_float)
+    tp = C.POINTER(PpgSdtree)
+    lib.ppg_export_sdtree.argtypes = [H, C.c_int, tp, f32p]
+    lib.ppg_op_dtree_pdf.argtypes = [C.c_int, tp, u32p, f32p, C.c_size_t, f32p]
+    lib.ppg_op_dtree_sample.argtypes = [C.c_int, tp, u32p, f32p, C.c_size_t, C.c_size_t, f32p, f32p]
+    lib.ppg_op_dtree_record.argtypes = [C.c_int, tp, u32p, f32p, f32p, f32p, f32p, C.c_size_t, C.c_int]
+    lib.ppg_op_stree_lookup.argtypes = [C.c_int, tp, f32p, f32p, f32p, C.c_size_t, u32p, f32p]
     lib.ppg_op_bvh_build.argtypes = [f32p, u32p, C.c_size_t, C.c_int, f32p, C.c_size_t, u32p, C.POINTER(C.c_size_t), C.POINTER(C.c_int), C.POINTER(C.c_double)]
     lib.ppg_op_emitter_sample_direct.argtypes = [H, C.c_size_t, f32p, f32p, f32p, C.c_int, f32p, f32p, f32p, f32p]
     lib.ppg_op_env_pdf.argtypes = [H, C.c_size_t, f32p, f32p, f32p]
-    i32p = C.POINTER(C.c_int32); u8p = C.POINTER(C.c_uint8); szp = C.POINTER(C.c_size_t); sz = C.c_size_t
-    lib.ppg_op_sdtree_refine_reset.argtypes = [C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, sz, u32p, sz, u32p, u32p, i32p, f32p, f32p, f32p, f32p, f32p, u16p, sz,
-                                               sz, szp, u32p, u32p, u32p, i32p, f32p, f32p, f32p, f32p, u32p, u32p, i32p, sz, szp, u16p, f32p]
-    lib.ppg_op_sdtree_build.argtypes = [C.c_int, u32p, sz, u32p, u32p, i32p, f32p, f32p, u16p, sz, f32p, u16p, f32p, f32p, i32p, u32p, u8p, C.POINTER(C.c_double)]
-    lib.ppg_op_commit.argtypes = [C.c_int, C.c_int, u32p, sz, f32p, f32p, u32p, f32p, f32p, u16p, sz, f32p, sz, f32p, sz, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_float,
-                                  f32p, sz, szp]
+    u8p = C.POINTER(C.c_uint8); szp = C.POINTER(C.c_size_t); sz = C.c_size_t
+    lib.ppg_op_sdtree_refine_reset.argtypes = [C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, sz, tp, f32p, tp, tp]
+    lib.ppg_op_sdtree_build.argtypes = [C.c_int, tp, tp, u8p, C.POINTER(C.c_double)]
+    lib.ppg_op_commit.argtypes = [C.c_int, C.c_int, tp, f32p, f32p, f32p, sz, f32p, sz, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_float, f32p, sz, szp]
     lib.ppg_op_adam_replay.argtypes = [C.c_int, C.c_int, C.c_int, f32p, sz, f32p, sz, u32p, u32p, f32p, f32p, u32p, u32p, u32p]
     if path is None:
         _lib = lib

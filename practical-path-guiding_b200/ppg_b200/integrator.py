@@ -154,17 +154,9 @@ class GuidedPathTracer:
         """The SD-tree as flat arrays (ppg_export_sdtree), after render() or from inside the film callback; which: 0 = sampling trees,
         1 = building trees.  Returns a dict: s_children (N, 2), tree_first / tree_count / tree_depth /
         tree_sum / tree_weight (N,), adam (N, 6), sums (M, 4), children (M, 4) uint16, aabb (2, 3)."""
-        nn, nq = C.c_size_t(), C.c_size_t()
-        rc = self.lib.ppg_export_sdtree(self._h, which, 0, C.byref(nn), None, None, None, None, None, None, None, 0, C.byref(nq), None, None, None)
-        _check(self.lib, rc, allow=(-1,) if nn.value or nq.value else ())      # -1 with the sizes filled in: the arrays were too small
-        N, M = nn.value, nq.value
-        e = dict(s_children=np.zeros((N, 2), np.uint32), tree_first=np.zeros(N, np.uint64), tree_count=np.zeros(N, np.uint32), tree_depth=np.zeros(N, np.int32),
-                 tree_sum=np.zeros(N, np.float32), tree_weight=np.zeros(N, np.float32), adam=np.zeros((N, 6), np.float32), sums=np.zeros((M, 4), np.float32),
-                 children=np.zeros((M, 4), np.uint16), aabb=np.zeros((2, 3), np.float32))
-        P = lambda k, t: e[k].ctypes.data_as(C.POINTER(t))
-        _check(self.lib, self.lib.ppg_export_sdtree(self._h, which, N, C.byref(nn), P("s_children", C.c_uint32), P("tree_first", C.c_uint64), P("tree_count", C.c_uint32),
-                                                    P("tree_depth", C.c_int32), P("tree_sum", C.c_float), P("tree_weight", C.c_float), P("adam", C.c_float),
-                                                    M, C.byref(nq), P("sums", C.c_float), P("children", C.c_uint16), P("aabb", C.c_float)))
+        aabb = np.zeros((2, 3), np.float32)
+        e, = _sized(self.lib, lambda t: self.lib.ppg_export_sdtree(self._h, which, t, _p(aabb, C.c_float)), [(0, 0)])
+        e["aabb"] = aabb
         return e
 
     def op_emitter_sample_direct(self, ref, ref_n, sample, max_interactions=-1):
@@ -214,40 +206,76 @@ def _p(a, t):
     return a.ctypes.data_as(C.POINTER(t))
 
 
+# ppg_sdtree (include/ppg.h) as a dict of arrays, keyed as GuidedPathTracer.export_sdtree returns them: key -> (field, C type, columns)
+_SDTREE = dict(s_children=("node_children", C.c_uint32, 2), tree_first=("tree_first", C.c_uint64, 1), tree_count=("tree_count", C.c_uint32, 1),
+               tree_depth=("tree_depth", C.c_int32, 1), tree_sum=("tree_sum", C.c_float, 1), tree_weight=("tree_weight", C.c_float, 1),
+               adam=("adam", C.c_float, 6), sums=("sums", C.c_float, 4), children=("children", C.c_uint16, 4))
+_POOL = ("sums", "children")
+
+
+def _sdtree(arrays):
+    """A ppg_sdtree over `arrays` (keys of _SDTREE; absent or None: NULL), sized and with room for their lengths.  The arrays are converted to
+    the C types in the dict, which the struct keeps alive as `.arrays`."""
+    t = capi.PpgSdtree()
+    for k, (field, ct, w) in _SDTREE.items():
+        if arrays.get(k) is None:
+            continue
+        a = arrays[k] = np.ascontiguousarray(arrays[k], ct).reshape((-1, w) if w > 1 else -1)
+        setattr(t, field, _p(a, ct))
+        if k in _POOL:
+            t.n_pool = t.pool_capacity = len(a)
+        else:
+            t.n_nodes = t.node_capacity = len(a)
+    t.arrays = arrays
+    return t
+
+
+def _sdtree_out(n_nodes, n_pool):
+    return _sdtree({k: np.zeros(((n_pool if k in _POOL else n_nodes), w) if w > 1 else n_nodes, ct) for k, (_, ct, w) in _SDTREE.items()})
+
+
+def _sized(lib, call, caps):
+    """call(*trees) with output trees of the capacities caps [(nodes, pool), ...], repeated once at the sizes it reports if they were too small.
+    Returns the trees' arrays, trimmed to their sizes."""
+    for _ in range(2):
+        outs = [_sdtree_out(n, m) for n, m in caps]
+        rc = call(*outs)
+        if rc != -1 or all(t.n_nodes <= n and t.n_pool <= m for t, (n, m) in zip(outs, caps)):
+            break
+        caps = [(max(n, t.n_nodes), max(m, t.n_pool)) for t, (n, m) in zip(outs, caps)]
+    _check(lib, rc)
+    return [{k: v[:t.n_pool] if k in _POOL else v[:t.n_nodes] for k, v in t.arrays.items()} for t in outs]
+
+
 def op_dtree_pdf(sums, children, tree_first, tree_sum, tree_weight, query_tree, query_dir, device=0):
     lib = capi.load_library()
-    sums = np.ascontiguousarray(sums, np.float32); children = np.ascontiguousarray(children, np.uint16)
-    tf = np.ascontiguousarray(tree_first, np.uint32); ts = np.ascontiguousarray(tree_sum, np.float32); tw = np.ascontiguousarray(tree_weight, np.float32)
+    t = _sdtree(dict(tree_first=tree_first, tree_sum=tree_sum, tree_weight=tree_weight, sums=sums, children=children))
     qt = np.ascontiguousarray(query_tree, np.uint32); qd = np.ascontiguousarray(query_dir, np.float32)
     out = np.zeros(len(qt), np.float32)
-    _check(lib, lib.ppg_op_dtree_pdf(device, _p(sums, C.c_float), _p(children, C.c_uint16), len(sums), _p(tf, C.c_uint32), _p(ts, C.c_float),
-                                     _p(tw, C.c_float), len(tf), _p(qt, C.c_uint32), _p(qd, C.c_float), len(qt), _p(out, C.c_float)))
+    _check(lib, lib.ppg_op_dtree_pdf(device, t, _p(qt, C.c_uint32), _p(qd, C.c_float), len(qt), _p(out, C.c_float)))
     return out
 
 
 def op_dtree_sample(sums, children, tree_first, tree_sum, tree_weight, query_tree, rnd, device=0, canonical=False):
     """Sampled directions (n, 3); with canonical=True also the points DTree::sample returns before canonicalToDir, (n, 2)."""
     lib = capi.load_library()
-    sums = np.ascontiguousarray(sums, np.float32); children = np.ascontiguousarray(children, np.uint16)
-    tf = np.ascontiguousarray(tree_first, np.uint32); ts = np.ascontiguousarray(tree_sum, np.float32); tw = np.ascontiguousarray(tree_weight, np.float32)
+    t = _sdtree(dict(tree_first=tree_first, tree_sum=tree_sum, tree_weight=tree_weight, sums=sums, children=children))
     qt = np.ascontiguousarray(query_tree, np.uint32); rnd = np.ascontiguousarray(rnd, np.float32)
     out = np.zeros((len(qt), 3), np.float32)
     canon = np.zeros((len(qt), 2), np.float32) if canonical else None
-    _check(lib, lib.ppg_op_dtree_sample(device, _p(sums, C.c_float), _p(children, C.c_uint16), len(sums), _p(tf, C.c_uint32), _p(ts, C.c_float),
-                                        _p(tw, C.c_float), len(tf), _p(qt, C.c_uint32), _p(rnd, C.c_float), rnd.shape[1], len(qt), _p(out, C.c_float),
+    _check(lib, lib.ppg_op_dtree_sample(device, t, _p(qt, C.c_uint32), _p(rnd, C.c_float), rnd.shape[1], len(qt), _p(out, C.c_float),
                                         None if canon is None else _p(canon, C.c_float)))
     return (out, canon) if canonical else out
 
 
 def op_dtree_record(sums, children, tree_first, tree_weight, rec_tree, rec_dir, rec_radiance, rec_wo_pdf, rec_weight, directional_filter=0, device=0):
     lib = capi.load_library()
-    sums = np.array(sums, np.float32, copy=True, order="C"); children = np.ascontiguousarray(children, np.uint16)
-    tf = np.ascontiguousarray(tree_first, np.uint32); tw = np.array(tree_weight, np.float32, copy=True, order="C")
+    t = _sdtree(dict(tree_first=tree_first, tree_weight=np.array(tree_weight, np.float32), sums=np.array(sums, np.float32), children=children))
     rt = np.ascontiguousarray(rec_tree, np.uint32); rd = np.ascontiguousarray(rec_dir, np.float32)
     rr = np.ascontiguousarray(rec_radiance, np.float32); rp = np.ascontiguousarray(rec_wo_pdf, np.float32); rw = np.ascontiguousarray(rec_weight, np.float32)
-    _check(lib, lib.ppg_op_dtree_record(device, _p(sums, C.c_float), _p(children, C.c_uint16), len(sums), _p(tf, C.c_uint32), _p(tw, C.c_float), len(tf),
-                                        _p(rt, C.c_uint32), _p(rd, C.c_float), _p(rr, C.c_float), _p(rp, C.c_float), _p(rw, C.c_float), len(rt), directional_filter))
-    return sums, tw
+    _check(lib, lib.ppg_op_dtree_record(device, t, _p(rt, C.c_uint32), _p(rd, C.c_float), _p(rr, C.c_float), _p(rp, C.c_float), _p(rw, C.c_float), len(rt),
+                                        directional_filter))
+    return t.arrays["sums"], t.arrays["tree_weight"]
 
 
 def _c(a, dt):
@@ -264,29 +292,16 @@ def op_sdtree_refine_reset(tree, building_weight, threshold, refine=True, reset=
     Returns a dict of the new S-tree: s_children, tree_first/count/depth/sum/weight, adam, building_weight (after the refine) and the new
     building trees: build_first/count/depth, build_children, build_sums."""
     lib = capi.load_library()
-    sch = _c(tree["s_children"], np.uint32); n = len(sch)
-    ins = [_c(tree["tree_first"], np.uint32), _c(tree["tree_count"], np.uint32), _c(tree["tree_depth"], np.int32), _c(tree["tree_sum"], np.float32),
-           _c(tree["tree_weight"], np.float32), _c(tree["adam"], np.float32), _c(building_weight, np.float32)]
-    sums = _c(tree["sums"], np.float32); ch = _c(tree["children"], np.uint16)
-    cap, bcap = max(2 * n, 1024), max(4 * len(sums), 1024)
-    nn, nb = C.c_size_t(), C.c_size_t()
-    for _ in range(2):
-        o = dict(s_children=np.zeros((cap, 2), np.uint32), tree_first=np.zeros(cap, np.uint32), tree_count=np.zeros(cap, np.uint32), tree_depth=np.zeros(cap, np.int32),
-                 tree_sum=np.zeros(cap, np.float32), tree_weight=np.zeros(cap, np.float32), adam=np.zeros((cap, 6), np.float32), building_weight=np.zeros(cap, np.float32),
-                 build_first=np.zeros(cap, np.uint32), build_count=np.zeros(cap, np.uint32), build_depth=np.zeros(cap, np.int32),
-                 build_children=np.zeros((bcap, 4), np.uint16), build_sums=np.zeros((bcap, 4), np.float32))
-        T = (C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_uint32, C.c_uint32, C.c_int32)
-        keys = ("s_children", "tree_first", "tree_count", "tree_depth", "tree_sum", "tree_weight", "adam", "building_weight", "build_first", "build_count", "build_depth")
-        rc = lib.ppg_op_sdtree_refine_reset(device, (1 if refine else 0) | (2 if reset else 0), threshold, new_max_depth, dtree_threshold, node_capacity,
-                                            _p(sch, C.c_uint32), n, *[_p(a, t) for a, t in zip(ins, (C.c_uint32, C.c_uint32, C.c_int32) + (C.c_float,) * 4)],
-                                            _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), cap, C.byref(nn), *[_p(o[k], t) for k, t in zip(keys, T)],
-                                            bcap, C.byref(nb), _p(o["build_children"], C.c_uint16), _p(o["build_sums"], C.c_float))
-        if rc == -1 and (nn.value > cap or nb.value > bcap):
-            cap, bcap = max(cap, nn.value), max(bcap, nb.value)
-            continue
-        _check(lib, rc)
-        break
-    o = {k: (v[:nb.value] if k in ("build_children", "build_sums") else v[:nn.value]) for k, v in o.items()}
+    t = _sdtree({k: tree.get(k) for k in _SDTREE})
+    bw = _c(building_weight, np.float32)
+    cap = max(2 * t.n_nodes, 1024)
+    s, b = _sized(lib, lambda s, b: lib.ppg_op_sdtree_refine_reset(device, (1 if refine else 0) | (2 if reset else 0), threshold, new_max_depth, dtree_threshold,
+                                                                   node_capacity, t, _p(bw, C.c_float), s, b),
+                  [(cap, t.n_pool), (cap, max(4 * t.n_pool, 1024))])
+    o = {k: s[k] for k in ("s_children", "tree_first", "tree_count", "tree_depth", "tree_sum", "tree_weight", "adam")}
+    o["tree_first"] = o["tree_first"].astype(np.uint32)
+    o.update(building_weight=b["tree_weight"], build_first=b["tree_first"].astype(np.uint32), build_count=b["tree_count"], build_depth=b["tree_depth"],
+             build_children=b["children"], build_sums=b["sums"])
     return o
 
 
@@ -294,18 +309,14 @@ def op_sdtree_build(s_children, build_first, build_count, build_depth, building_
     """DTree::build of every leaf + "sampling = building" + the distribution statistics through the render's kernels (ppg_op_sdtree_build).
     Returns (sampling sums, sampling children, dict of per-node tree_sum / tree_weight / tree_depth / tree_count / mean_positive, stats dict)."""
     lib = capi.load_library()
-    sch = _c(s_children, np.uint32); n = len(sch)
-    bf, bc, bd, bw = _c(build_first, np.uint32), _c(build_count, np.uint32), _c(build_depth, np.int32), _c(building_weight, np.float32)
-    sums = _c(sums, np.float32); ch = _c(children, np.uint16)
-    ss, sc = np.zeros_like(sums), np.zeros_like(ch)
-    per = dict(tree_sum=np.zeros(n, np.float32), tree_weight=np.zeros(n, np.float32), tree_depth=np.zeros(n, np.int32), tree_count=np.zeros(n, np.uint32),
-               mean_positive=np.zeros(n, np.uint8))
-    st = np.zeros(14, np.float64)
-    _check(lib, lib.ppg_op_sdtree_build(device, _p(sch, C.c_uint32), n, _p(bf, C.c_uint32), _p(bc, C.c_uint32), _p(bd, C.c_int32), _p(bw, C.c_float),
-                                        _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), _p(ss, C.c_float), _p(sc, C.c_uint16),
-                                        _p(per["tree_sum"], C.c_float), _p(per["tree_weight"], C.c_float), _p(per["tree_depth"], C.c_int32),
-                                        _p(per["tree_count"], C.c_uint32), _p(per["mean_positive"], C.c_uint8), _p(st, C.c_double)))
-    return ss, sc, per, dict(zip(TREE_STATS, st.tolist()))
+    b = _sdtree(dict(s_children=s_children, tree_first=build_first, tree_count=build_count, tree_depth=build_depth, tree_weight=building_weight, sums=sums,
+                     children=children))
+    s = _sdtree_out(b.n_nodes, b.n_pool)
+    mp = np.zeros(b.n_nodes, np.uint8); st = np.zeros(14, np.float64)
+    _check(lib, lib.ppg_op_sdtree_build(device, b, s, _p(mp, C.c_uint8), _p(st, C.c_double)))
+    e = s.arrays
+    per = dict(tree_sum=e["tree_sum"], tree_weight=e["tree_weight"], tree_depth=e["tree_depth"], tree_count=e["tree_count"], mean_positive=mp)
+    return e["sums"], e["children"], per, dict(zip(TREE_STATS, st.tolist()))
 
 
 def op_commit(s_children, aabb_min, aabb_extent, build_first, building_weight, sums, children, vertices, li_final, record_mode=2, spatial_filter=0,
@@ -313,15 +324,15 @@ def op_commit(s_children, aabb_min, aabb_extent, build_first, building_weight, s
     """Vertex::commit of the vertices (n, 6, 4) float32 -- the six float4 the bounce kernel writes -- through the render's commit kernel
     (ppg_op_commit).  Returns (building sums, building weights, sampling-fraction records (m, 6) float32 with the leaf's bits in column 0)."""
     lib = capi.load_library()
-    sch = _c(s_children, np.uint32); mn = _c(aabb_min, np.float32); ex = _c(aabb_extent, np.float32); bf = _c(build_first, np.uint32)
-    bw = np.array(building_weight, np.float32, copy=True, order="C"); sums = np.array(sums, np.float32, copy=True, order="C"); ch = _c(children, np.uint16)
+    t = _sdtree(dict(s_children=s_children, tree_first=build_first, tree_weight=np.array(building_weight, np.float32), sums=np.array(sums, np.float32),
+                     children=children))
+    mn = _c(aabb_min, np.float32); ex = _c(aabb_extent, np.float32)
     v = _c(vertices, np.float32).reshape(-1, 24); li = _c(li_final, np.float32).reshape(-1, 4)
     cap = len(v) * 64 if adam_capacity is None else adam_capacity
     rec = np.zeros((max(cap, 1), 6), np.float32); na = C.c_size_t()
-    _check(lib, lib.ppg_op_commit(device, record_mode, _p(sch, C.c_uint32), len(sch), _p(mn, C.c_float), _p(ex, C.c_float), _p(bf, C.c_uint32), _p(bw, C.c_float),
-                                  _p(sums, C.c_float), _p(ch, C.c_uint16), len(sums), _p(v, C.c_float), len(v), _p(li, C.c_float), len(li), spatial_filter,
-                                  directional_filter, loss, seed, statistical_weight, _p(rec, C.c_float), cap, C.byref(na)))
-    return sums, bw, rec[:min(na.value, cap)]
+    _check(lib, lib.ppg_op_commit(device, record_mode, t, _p(mn, C.c_float), _p(ex, C.c_float), _p(v, C.c_float), len(v), _p(li, C.c_float), len(li),
+                                  spatial_filter, directional_filter, loss, seed, statistical_weight, _p(rec, C.c_float), cap, C.byref(na)))
+    return t.arrays["sums"], t.arrays["tree_weight"], rec[:min(na.value, cap)]
 
 
 def op_adam_replay(state, records, loss, leaf_offset=None, leaf_count=None, bucket=False, device=0):
@@ -353,9 +364,8 @@ def op_bvh_build(positions, indices, threads=0):
 
 def op_stree_lookup(node_children, aabb_min, aabb_extent, points, device=0):
     lib = capi.load_library()
-    nc = np.ascontiguousarray(node_children, np.uint32); pts = np.ascontiguousarray(points, np.float32)
-    mn = np.ascontiguousarray(aabb_min, np.float32); ex = np.ascontiguousarray(aabb_extent, np.float32)
+    t = _sdtree(dict(s_children=node_children))
+    pts = np.ascontiguousarray(points, np.float32); mn = np.ascontiguousarray(aabb_min, np.float32); ex = np.ascontiguousarray(aabb_extent, np.float32)
     leaf = np.zeros(len(pts), np.uint32); size = np.zeros((len(pts), 3), np.float32)
-    _check(lib, lib.ppg_op_stree_lookup(device, _p(nc, C.c_uint32), len(nc), _p(mn, C.c_float), _p(ex, C.c_float), _p(pts, C.c_float), len(pts),
-                                        _p(leaf, C.c_uint32), _p(size, C.c_float)))
+    _check(lib, lib.ppg_op_stree_lookup(device, t, _p(mn, C.c_float), _p(ex, C.c_float), _p(pts, C.c_float), len(pts), _p(leaf, C.c_uint32), _p(size, C.c_float)))
     return leaf, size

@@ -20,17 +20,17 @@ def test_library_exports_every_declared_symbol():
     for s in declared:
         assert hasattr(lib, s), s
     assert lib.ppg_description() == b"Guided path tracer"      # MTS_EXPORT_PLUGIN(GuidedPathTracer, "Guided path tracer"), GP:2422
-    assert lib.ppg_abi_version() == 2
+    assert lib.ppg_abi_version() == 3
 
 
 def test_struct_layouts_match_header():
-    src = '#include "%s"\n#include <stdio.h>\nint main(){printf("%%zu %%zu %%zu %%zu %%zu %%zu %%zu", sizeof(ppg_params), sizeof(ppg_bsdf), sizeof(ppg_shape), sizeof(ppg_scene_desc), sizeof(ppg_iteration_stats), sizeof(ppg_stats), sizeof(ppg_sphere));}' % os.path.join(ROOT, "include", "ppg.h")
+    src = '#include "%s"\n#include <stdio.h>\nint main(){printf("%%zu %%zu %%zu %%zu %%zu %%zu %%zu %%zu", sizeof(ppg_params), sizeof(ppg_bsdf), sizeof(ppg_shape), sizeof(ppg_scene_desc), sizeof(ppg_iteration_stats), sizeof(ppg_stats), sizeof(ppg_sphere), sizeof(ppg_sdtree));}' % os.path.join(ROOT, "include", "ppg.h")
     import subprocess, tempfile
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "s.c"), "w").write(src)
         subprocess.run(["/usr/bin/gcc", os.path.join(d, "s.c"), "-o", os.path.join(d, "s")], check=True)
         sizes = [int(x) for x in subprocess.run([os.path.join(d, "s")], capture_output=True, text=True, check=True).stdout.split()]
-    assert sizes == [C.sizeof(capi.PpgParams), C.sizeof(capi.PpgBsdf), C.sizeof(capi.PpgShape), C.sizeof(capi.PpgSceneDesc), C.sizeof(capi.PpgIterationStats), C.sizeof(capi.PpgStats), C.sizeof(capi.PpgSphere)]
+    assert sizes == [C.sizeof(capi.PpgParams), C.sizeof(capi.PpgBsdf), C.sizeof(capi.PpgShape), C.sizeof(capi.PpgSceneDesc), C.sizeof(capi.PpgIterationStats), C.sizeof(capi.PpgStats), C.sizeof(capi.PpgSphere), C.sizeof(capi.PpgSdtree)]
     assert C.sizeof(capi.PpgBsdf) == 112 and C.sizeof(capi.PpgSphere) == 24
 
 
