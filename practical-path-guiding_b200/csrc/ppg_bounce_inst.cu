@@ -1,7 +1,6 @@
 // ppg_bounce_inst.cu -- one (SMEM, FULL) family of bounce_kernel instantiations per translation unit:
 //   nvcc -DPPG_INST_SMEM={0,1} -DPPG_INST_FULL={0,1} -c ppg_bounce_inst.cu
 #include "ppg_bounce.cuh"
-#include <cstdlib>
 
 using namespace ppg;
 
@@ -13,14 +12,8 @@ using namespace ppg;
 namespace {
 constexpr bool kSmem = PPG_INST_SMEM != 0, kFull = PPG_INST_FULL != 0;
 constexpr int kBlock = kSmem ? PPG_BOUNCE_BLOCK : PPG_BOUNCE_BLOCK_HBM;
-template <class K> void carveout(K kernel) {      // tuning experiments only
-    static const int pct = [] { const char *v = getenv("PPG_SMEM_CARVEOUT"); return v && *v ? atoi(v) : -1; }();
-    if (pct >= 0) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-}
 template <bool FIRST> void launch(const RenderParams &P, const BounceLaunch &L) {
     const size_t sm = P.sceneSmemBytes;
-    carveout(bounce_kernel<FIRST, 0, true, kSmem, kFull>); carveout(bounce_kernel<FIRST, 2, true, kSmem, kFull>); carveout(bounce_kernel<FIRST, 0, false, kSmem, kFull>);
-    carveout(bounce_kernel<FIRST, 1, false, kSmem, kFull>); carveout(bounce_kernel<FIRST, 2, false, kSmem, kFull>);
     if (L.nee) {      // next event estimation always runs with full records
         if (L.record == 0) bounce_kernel<FIRST, 0, true, kSmem, kFull><<<L.grid, kBlock, sm, L.stream>>>(P);
         else bounce_kernel<FIRST, 2, true, kSmem, kFull><<<L.grid, kBlock, sm, L.stream>>>(P);

@@ -1057,9 +1057,7 @@ __device__ __forceinline__ float sum4(float4 s, int i) { return i == 0 ? s.x : (
 // Table entry: node | levels<<24 | leaf<<31 (built by stree_table_kernel after every refine).  The node number has 24 bits, so the
 // table serves S-trees of at most 0xFFFFFF nodes (stree_table_usable); a larger tree is looked up with table == nullptr, the plain
 // walk from the root, which is the reference's walk and returns the same leaf bit for bit.
-#ifndef PPG_STREE_TABLE_BITS
-#define PPG_STREE_TABLE_BITS 7                     // digits per axis -> 3*7 = 21 levels, 2^21 entries (8 MB, L2 resident; CBOX 1024^2 descends 18.5 levels on average)
-#endif
+constexpr int PPG_STREE_TABLE_BITS = 7;     // digits per axis -> 3*7 = 21 levels, 2^21 entries (8 MB, L2 resident; CBOX 1024^2 descends 18.5 levels on average)
 // whether stree_table_kernel's entries can hold every node number of an S-tree of n_nodes nodes (host side: pass the table or nullptr)
 inline bool stree_table_usable(size_t n_nodes) { return n_nodes <= 0x00ffffffu; }
 __device__ __forceinline__ uint32_t spread3(uint32_t v) {   // bit i -> bit 3i (7 bits)

@@ -47,8 +47,6 @@ static void wald_constants(H3 A, H3 B, H3 C, float out[9], int &k) {
     out[7] = hcomp(c, v) / denom; out[8] = -hcomp(c, u) / denom;                          // c_nu c_nv
 }
 
-static int env_int(const char *name, int dflt) { const char *v = getenv(name); return v && *v ? atoi(v) : dflt; }   // tuning experiments only
-
 // Host-side parallelism of the packing (per-triangle tables, BVH build, texel repacking): plain std::thread fork / join over index ranges.
 // Every parallel loop below computes exactly what its serial form computes (min / max / integer counts / independent elements), so the
 // scene tables do not depend on the thread count.
@@ -66,7 +64,7 @@ template <class F> static void parallel_for(size_t n, int threads, size_t minChu
     for (auto &th : pool) th.join();
 }
 
-// Binned-SAH BVH (16 bins per axis, leaves of at most PPG_BVH_LEAF triangles, a traversal-cost term decides the last splits).
+// Binned-SAH BVH (16 bins per axis, leaves of at most 4 triangles, a traversal-cost term decides the last splits).
 // The tree is a function of the triangle bounds alone: a node's split depends only on the triangles of its range, children work on disjoint
 // ranges of `order`.  It is therefore built in any order -- big nodes one after the other with their O(n) loops spread over the threads, the
 // subtrees below them concurrently -- into an arena, and numbered afterwards in the order a depth-first stack visits it (right child first),
@@ -79,8 +77,9 @@ static void build_bvh_from_bounds(const std::vector<H3> &tminV, const std::vecto
     parallel_for(nt, threads, 1 << 15, [&](size_t b, size_t e, int) {
         for (size_t t = b; t < e; ++t) { out.order[t] = (uint32_t) t; cen[t] = h3(0.5f * (tmin[t].x + tmax[t].x), 0.5f * (tmin[t].y + tmax[t].y), 0.5f * (tmin[t].z + tmax[t].z)); }
     });
-    const int maxLeaf = std::min(std::max(env_int("PPG_BVH_LEAF", 4), 1), 15);   // <= 15: the device stack packs the count in 4 bits
-    const float Ct = (float) env_int("PPG_BVH_CT_X10", 10) * 0.1f;
+    constexpr int maxLeaf = 4;
+    static_assert(maxLeaf >= 1 && maxLeaf <= 15, "the device stack packs a leaf's triangle count in 4 bits");
+    constexpr float Ct = 1.0f;                                                         // traversal cost, in triangle tests
     constexpr int NB = 16;
     struct Node { H3 mn, mx; uint32_t left, count; };                                 // count == 0: inner node, `left` = arena index of its first child
     struct Job { uint32_t node, first, count; int depth; };
@@ -295,7 +294,8 @@ static int validate(const ppg_scene_desc &s, std::string &error) {
 
 int host_threads() {
     static const int n = [] {
-        int t = env_int("PPG_HOST_THREADS", 0);
+        const char *e = getenv("PPG_HOST_THREADS");
+        int t = e && *e ? atoi(e) : 0;
         if (t <= 0) {
             t = (int) std::thread::hardware_concurrency();
 #ifdef __linux__

@@ -15,18 +15,10 @@
 
 namespace ppg {
 
-#ifndef PPG_TRACE_BLOCK
-#define PPG_TRACE_BLOCK 256
-#endif
-#ifndef PPG_TRACE_MIN_BLOCKS
-#define PPG_TRACE_MIN_BLOCKS 4
-#endif
-#ifndef PPG_TRACE_REFILL
-#define PPG_TRACE_REFILL 8u        // idle lanes that trigger a refill (one atomic per refill and warp)
-#endif
-#ifndef PPG_TRACE_STEPS
-#define PPG_TRACE_STEPS 16         // inner-node steps a lane may take before the warp looks at leaves / refills again
-#endif
+constexpr int PPG_TRACE_BLOCK = 256;
+constexpr int PPG_TRACE_MIN_BLOCKS = 4;
+constexpr unsigned PPG_TRACE_REFILL = 8u;    // idle lanes that trigger a refill (one atomic per refill and warp)
+constexpr int PPG_TRACE_STEPS = 16;          // inner-node steps a lane may take before the warp looks at leaves / refills again
 
 template <bool FIRST, bool SPHERES>
 __global__ void __launch_bounds__(PPG_TRACE_BLOCK, PPG_TRACE_MIN_BLOCKS) trace_kernel(const __grid_constant__ RenderParams P) {

@@ -13,25 +13,15 @@
 
 namespace ppg {
 
-#ifndef PPG_BLOCK
-#define PPG_BLOCK 256
-#endif
-#ifndef PPG_BOUNCE_BLOCK
-#define PPG_BOUNCE_BLOCK 1024          // threads per block of the bounce kernel: one block per SM stages the scene once (measured 256x4 -> 5589, 512x2 -> 5643,
-#endif                                 // 1024x1 -> 5676 Msamples/s on CBOX 1024^2)
-#ifndef PPG_BOUNCE_BLOCK_HBM
-#define PPG_BOUNCE_BLOCK_HBM 256       // scenes that do not fit shared memory (nothing to stage) keep 256 x 4: SPACESHIP 485 vs 450 Msamples/s of bounce-kernel time,
-#endif                                 // 269 vs 232 with the kl loss; the staged CBOX variants gain 1-4 % from 1024 x 1
-#ifndef PPG_MIN_BLOCKS
-#define PPG_MIN_BLOCKS 1               // resident blocks per SM the bounce kernel is compiled for: 1024 threads x 64 registers = the whole register file
-#endif
-#ifndef PPG_CLAIM
-#define PPG_CLAIM 1u                   // groups of 32 paths a warp claims per atomic (measured on CBOX 1024^2: 1 -> 5585, 4 -> 5385, 16 -> 4819 Msamples/s:
-                                       // running warps then sweep ONE contiguous window of the SoA path state)
-#endif
-#ifndef PPG_MIN_BLOCKS_HBM
-#define PPG_MIN_BLOCKS_HBM 4           // 64 registers as well (beat 80 and 128 on the rough CBOX variants)
-#endif
+constexpr int PPG_BLOCK = 256;
+constexpr int PPG_BOUNCE_BLOCK = 1024;       // threads per block of the bounce kernel: one block per SM stages the scene once (measured 256x4 -> 5589, 512x2 -> 5643,
+                                             // 1024x1 -> 5676 Msamples/s on CBOX 1024^2)
+constexpr int PPG_BOUNCE_BLOCK_HBM = 256;    // scenes that do not fit shared memory (nothing to stage) keep 256 x 4: SPACESHIP 485 vs 450 Msamples/s of bounce-kernel time,
+                                             // 269 vs 232 with the kl loss; the staged CBOX variants gain 1-4 % from 1024 x 1
+constexpr int PPG_MIN_BLOCKS = 1;            // resident blocks per SM the bounce kernel is compiled for: 1024 threads x 64 registers = the whole register file
+constexpr unsigned PPG_CLAIM = 1u;           // groups of 32 paths a warp claims per atomic (measured on CBOX 1024^2: 1 -> 5585, 4 -> 5385, 16 -> 4819 Msamples/s:
+                                             // running warps then sweep ONE contiguous window of the SoA path state)
+constexpr int PPG_MIN_BLOCKS_HBM = 4;        // 64 registers as well (beat 80 and 128 on the rough CBOX variants)
 #define PPG_MAX_VERTICES 32         // MAX_NUM_VERTICES, GP:1771
 #define PPG_INVALID 0xFFFFFFFFu
 

@@ -506,7 +506,7 @@ def test_spaceship_known_answers_of_the_reference_log():
     for k in (1, 2, 3):
         # The estimate sums min(luminance variance, 1e4) over the pixels (GP:1298-1319): ONE firefly pixel that reaches the clamp adds
         # 1e4 / (W H (N - 1)) = 0.043 / 0.014 / 0.006 at N = 2 / 4 / 8 samples, 44 % of the logged value of iteration 1.  Eight seeds
-        # (tools/perm_check.py) gave 0.091 - 0.106 against the log's 0.0976; a run with such a pixel gave 0.123.  Hence 15 % plus one clamped pixel.
+        # gave 0.091 - 0.106 against the log's 0.0976; a run with such a pixel gave 0.123.  Hence 15 % plus one clamped pixel.
         firefly = 1e4 / (640 * 360 * (it[k]["passes"] - 1))
         assert -0.15 * gold[k]["var"] <= it[k]["variance"] - gold[k]["var"] <= 0.15 * gold[k]["var"] + firefly, report
         assert abs(it[k]["weight_avg"] - gold[k]["stat_weight"][1]) <= 0.06 * gold[k]["stat_weight"][1], report

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """GPU box: sampling-fraction learning (kl) of the CUDA path against the authors' logs and the oracle.
-usage: learning_check.py [spaceship|kitchen] [repeats]   (env PPG_LOSS_GROWTH_PCT / PPG_LOSS_LEAF_PATHS_X10 tune the sub-batch schedule)"""
+usage: learning_check.py [spaceship|kitchen] [repeats]"""
 import json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "practical-path-guiding_b200")); sys.path.insert(0, os.path.join(ROOT, "tests"))
